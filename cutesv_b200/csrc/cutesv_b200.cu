@@ -113,8 +113,8 @@ struct LaneWork {
     cudaStream_t stream = nullptr;
     cudaEvent_t ev_join = nullptr;
     bool used = false;
-    DBuf keys_a, keys_b, vals_a, vals_b, hist, lb_status, bkt, bkt_flags, big_list, giant_list, giant_arena;
-    DBuf boff, rec_a, rec_b, recc_a, recc_b, big_bkt, rest_list;   // filter-first INS/DEL front end, k_cluster_small's rest list
+    DBuf keys_a, keys_b, vals_a, vals_b, hist, lb_status, big_list, giant_list, giant_arena;
+    DBuf boff, rec_a, rec_b, recc_a, recc_b, rest_list;   // partitioned INS/DEL front end, k_cluster_small's rest list
     SmallWork small;
 };
 static constexpr int N_LANES = CSV_NTYPES;
@@ -148,16 +148,14 @@ struct csv_ctx {
     int64_t n_aln = 0;
     DBuf a_chrom, a_start, a_end, a_id, a_prim, a_off, a_span;
     // sort workspace
-    DBuf keys_a, keys_b, vals_a, vals_b, hist, lb_status, tickets, bkt, bkt_flags;
-    DBuf boff, rec_a, rec_b, recc_a, recc_b, big_bkt;   // filter-first INS/DEL front end (per lane, see LaneWork)
+    DBuf keys_a, keys_b, vals_a, vals_b, hist, lb_status, tickets;
+    DBuf boff, rec_a, rec_b, recc_a, recc_b;   // partitioned INS/DEL front end (per lane, see LaneWork)
     DBuf rest_list;                  // kept clusters k_cluster_small left to the general kernel (per lane)
     DBuf scan_carry, emit_cursor;
     DBuf d_epoch;                    // look-back generation base, bumped by the first kernel of every csv_cluster
     uint32_t epoch_host = 0;
     bool small_chain[CSV_NTYPES] = {false, false, false, false, false};   // chained-sorts fallback after ST_BIG_RUN
     bool prefilter_enabled = true;
-    bool bucket_sort_enabled = true;
-    int64_t l2_bytes = 0;               // device L2 size: the density filter needs its bucket histogram to stay there
     bool records_enabled = true;
     bool small_path_enabled = true;
     int64_t pair_cap_override = 0;
@@ -410,7 +408,6 @@ extern "C" int csv_create(int device, void* stream, csv_ctx** out) {
     csv_ctx* c = new csv_ctx();
     c->device = device;
     c->n_sm = prop.multiProcessorCount;
-    c->l2_bytes = prop.l2CacheSize;
     if (stream) { c->stream = (cudaStream_t)stream; c->own_stream = false; }
     else {
         cudaError_t e2 = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
@@ -442,7 +439,6 @@ extern "C" int csv_create(int device, void* stream, csv_ctx** out) {
     if (const char* e = getenv("CUTESV_B200_GRAPHS")) c->graphs_enabled = atoi(e) != 0;
     if (const char* e = getenv("CUTESV_B200_PDL")) c->pdl_enabled = atoi(e) != 0;
     if (const char* e = getenv("CUTESV_B200_GATHER")) c->p2p_enabled = strcmp(e, "nccl") != 0;
-    if (const char* e = getenv("CUTESV_B200_BUCKET_SORT")) c->bucket_sort_enabled = atoi(e) != 0;
     if (const char* e = getenv("CUTESV_B200_RECORDS")) c->records_enabled = atoi(e) != 0;
     if (const char* e = getenv("CUTESV_B200_SMALL_PATH")) c->small_path_enabled = atoi(e) != 0;
     if (const char* e = getenv("CUTESV_B200_SMALL_CHAIN")) for (int t = 0; t < CSV_NTYPES; t++) c->small_chain[t] = atoi(e) != 0;
@@ -467,6 +463,7 @@ extern "C" int csv_create(int device, void* stream, csv_ctx** out) {
     CU(cudaFuncSetAttribute(k_cluster_block<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, BLOCK_M * ARENA_PER_MAX));
     CU(cudaFuncSetAttribute(k_cluster_block<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, BLOCK_M * ARENA_PER_MAX));
     CU(cudaFuncSetAttribute(k_cluster_block<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, BLOCK_M * ARENA_PER_MAX));
+    CU(cudaFuncSetAttribute(k_part_filter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pf_smem_bytes(PART_W_MAX)));
     *out = c;
     return CSV_OK;
 }
@@ -476,11 +473,11 @@ extern "C" int csv_destroy(csv_ctx* c) {
     cudaSetDevice(c->device);
     cudaStreamSynchronize(c->stream);
     DBuf* all[] = {&c->a_chrom, &c->a_start, &c->a_end, &c->a_id, &c->a_prim, &c->a_off, &c->a_span, &c->d_off, &c->d_len, &c->r_chrom, &c->r_start, &c->r_end, &c->r_id, &c->r_prim, &c->keys_a, &c->keys_b,
-                   &c->vals_a, &c->vals_b, &c->hist, &c->lb_status, &c->tickets, &c->bkt, &c->bkt_flags, &c->big_list, &c->giant_list, &c->giant_arena,
+                   &c->vals_a, &c->vals_b, &c->hist, &c->lb_status, &c->tickets, &c->big_list, &c->giant_list, &c->giant_arena,
                    &c->cnt, &c->cand_tmp, &c->cand, &c->geno, &c->names, &c->counters, &c->bin_start, &c->bin_fill, &c->bin_bits, &c->pairs, &c->win_list,
                    &c->dr, &c->has_rows, &c->gl_table, &c->pow_half, &c->small.k_rid, &c->small.k_b, &c->small.k_prim,
                    &c->small.perm_a, &c->small.perm_b, &c->small.sel, &c->small.u_chrom, &c->small.u_a, &c->small.u_b,
-                   &c->small.u_rid, &c->small.u_c, &c->boff, &c->rec_a, &c->rec_b, &c->recc_a, &c->recc_b, &c->big_bkt, &c->d_epoch,
+                   &c->small.u_rid, &c->small.u_c, &c->boff, &c->rec_a, &c->rec_b, &c->recc_a, &c->recc_b, &c->d_epoch,
                    &c->d_len_eff, &c->g_send, &c->g_recv, &c->g_cand, &c->g_geno, &c->g_names, &c->g_scratch, &c->g_tab, &c->cal_in0, &c->cal_in1,
                    &c->cal_out, &c->aln_flag, &c->scan_carry, &c->win_rec, &c->rest_list, &c->emit_cursor};
     for (DBuf* b : all) b->release();
@@ -491,8 +488,8 @@ extern "C" int csv_destroy(csv_ctx* c) {
         LaneWork& L = c->lanes[l];
         if (L.stream) { cudaStreamSynchronize(L.stream); cudaStreamDestroy(L.stream); }
         if (L.ev_join) cudaEventDestroy(L.ev_join);
-        DBuf* lb[] = {&L.keys_a, &L.keys_b, &L.vals_a, &L.vals_b, &L.hist, &L.lb_status, &L.bkt, &L.bkt_flags, &L.big_list, &L.giant_list, &L.giant_arena,
-                      &L.boff, &L.rec_a, &L.rec_b, &L.recc_a, &L.recc_b, &L.big_bkt, &L.rest_list,
+        DBuf* lb[] = {&L.keys_a, &L.keys_b, &L.vals_a, &L.vals_b, &L.hist, &L.lb_status, &L.big_list, &L.giant_list, &L.giant_arena,
+                      &L.boff, &L.rec_a, &L.rec_b, &L.recc_a, &L.recc_b, &L.rest_list,
                       &L.small.k_rid, &L.small.k_b, &L.small.k_prim, &L.small.perm_a, &L.small.perm_b, &L.small.sel, &L.small.u_chrom, &L.small.u_a,
                       &L.small.u_b, &L.small.u_rid, &L.small.u_c};
         for (DBuf* b : lb) b->release();
@@ -756,16 +753,14 @@ static int make_sync(csv_ctx* c, size_t status_words, TileSync* ts) {
 // ------------------------------------------------------------------------------------------
 template <typename K>
 static int radix_sort(csv_ctx* c, K* keys_a, uint32_t* vals_a, K* keys_b, uint32_t* vals_b, bool iota, int64_t n,
-                      const uint32_t* n_dev, int bits, K** keys_out, uint32_t** vals_out, int dom_type = -1, bool hist_ready = false) {
+                      const uint32_t* n_dev, int bits, K** keys_out, uint32_t** vals_out, int dom_type = -1) {
     const int passes = std::max(1, (bits + 7) / 8);
     if (passes > RS_MAX_PASSES) return set_err(CSV_E_INVALID, "radix sort: %d bits", bits);
     constexpr int TILE = RS_THREADS * RsTraits<K>::ITEMS;
     const int64_t n_tiles = (n + TILE - 1) / TILE;
     CU(c->hist.ensure(RS_MAX_PASSES * 256 * 4));
-    if (!hist_ready) {   // (the density pre-filter already counted the digits of its survivors)
-        CU(cudaMemsetAsync(c->hist.p, 0, RS_MAX_PASSES * 256 * 4, c->stream));
-        LAUNCH(c, (k_rs_hist<K>), grid_for(c, n, RS_THREADS * 16, 4), RS_THREADS, 0, keys_a, n, n_dev, passes, c->hist.as<uint32_t>());
-    }
+    CU(cudaMemsetAsync(c->hist.p, 0, RS_MAX_PASSES * 256 * 4, c->stream));
+    LAUNCH(c, (k_rs_hist<K>), grid_for(c, n, RS_THREADS * 16, 4), RS_THREADS, 0, keys_a, n, n_dev, passes, c->hist.as<uint32_t>());
     LAUNCH(c, k_rs_hist_scan, 1, 256, 0, c->hist.as<uint32_t>(), passes);
     K* ki = keys_a; K* ko = keys_b;
     uint32_t* vi = vals_a; uint32_t* vo = vals_b;
@@ -851,7 +846,7 @@ static int run_segment_and_cluster(csv_ctx* c, TypeJob& J, int t, uint32_t kslot
                 J.small_list = MR.small_list; J.n_small = MR.n_small; J.rest_list = MR.rest_list; J.n_rest = MR.n_rest;
             }
         }
-        if (c->prev_is_chain_kernel)   // directly behind k_bucket_fixup on this stream
+        if (c->prev_is_chain_kernel)   // directly behind k_part_filter on this stream
             LAUNCH_PDL(c, k_select_heads, grid_for(c, J.n_host, SEL_TILE, 4), SEL_THREADS, 0, J, c->kept[t].as<uint32_t>(), c->kept_cap[t],
                        &ctr->n_kept[t], ts, &ctr->status, (uint32_t)ST_LIST_OVERFLOW, MR);
         else
@@ -928,86 +923,65 @@ static int run_indel(csv_ctx* c, int t, uint32_t kslot_base) {
     const uint32_t radius = (uint32_t)std::min<int64_t>((int64_t)(J.cp.min_support - 1) * J.cp.bias, 1 << 24);
     const double lambda = (double)n * (2.0 * radius + 2.0 * (1 << BKT_SHIFT)) / (double)std::max<uint64_t>(total, 1);
     const int rb = (int)((radius + (1u << BKT_SHIFT) - 1) >> BKT_SHIFT);  // neighbourhood radius in buckets (conservative)
-    const size_t n_bkt = (((size_t)(total >> BKT_SHIFT) + 4096) / 4096 + 1) * 4096 + 3 * BKT_PAD + 64;
-    // The filter takes one scattered atomic per signature into the 4 B-per-bucket histogram; that only pays while the
-    // histogram stays in L2.  A whole human genome's (48 MB) does not fit beside the streams in an H100's 50 MB L2: there
-    // the plain sort of every signature is faster (config 2, H100: 1.52 ms/step vs 2.13 with the filter).
-    const bool hist_fits_l2 = (int64_t)(n_bkt * 4) <= c->l2_bytes / 2;
     const bool prefilter = !k64 && c->prefilter_enabled && J.cp.min_support >= 3 && lambda < 0.8 * J.cp.min_support &&
-                           n >= (1 << 16) && rb <= BKT_PAD && hist_fits_l2;
-    const bool bucket_sort = prefilter && c->bucket_sort_enabled;
+                           n >= (1 << 16) && rb <= BKT_PAD;
     J.iv.rec = nullptr; J.iv.recc = nullptr;
     uint32_t* sidx = nullptr;
     int rc;
-    if (bucket_sort) {
-        // filter-first front end: histogram -> flags + slot offsets -> scatter of (key, index) -> in-bucket order
-        const uint32_t n_buckets = (uint32_t)(total >> BKT_SHIFT) + 1;
-        const uint32_t n_tiles = (n_buckets + BP_TILE - 1) / BP_TILE;
+    if (prefilter) {
+        // filter-first front end, partitioned by genome range: count -> scan -> scatter of (key, index) by partition ->
+        // per partition, in shared memory: bucket histogram, density flags, survivors in key order.  W: the widest
+        // partitions (at most 2^22 bp) that still give every SM about two of them.
+        int W = PART_W_MAX;
+        while (W > PART_W_MIN && (int64_t)(total >> W) + 1 < 2 * (int64_t)c->n_sm) W--;
+        const int P = (int)(total >> W) + 1;
+        const int n_chunks = (int)((n + PART_CHUNK - 1) / PART_CHUNK);
+        const size_t cnt_words = (size_t)P * n_chunks, edge_words = (size_t)P * 2 * BKT_PAD;
         stage_begin(c, CSV_ST_KEYS);
-        CU(c->bkt.ensure(n_bkt * 4, true));   // all-zero between calls: zeroed when (re)allocated, cleared again by k_bucket_fixup
-        CU(c->boff.ensure(((size_t)n_tiles * BP_TILE + (size_t)n_tiles + 64) * 4));   // bpre[n_tiles * BP_TILE] | tile totals -> bases
-        const uint32_t bb_cap = (uint32_t)(n / FIX_SMALL + 2);
-        CU(c->big_bkt.ensure((size_t)bb_cap * sizeof(uint4)));
-        uint32_t* bpre = c->boff.as<uint32_t>();
-        uint32_t* tile_base = bpre + (size_t)n_tiles * BP_TILE;
-        LAUNCH(c, k_indel_hist, grid_for(c, n, 256 * 4), 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), n, t == CSV_INS ? 1 : 0, ct,
-               &ctr->status, c->bkt.as<uint32_t>());
-        uint32_t* n_pass = &ctr->n_dom[t];
+        CU(c->boff.ensure((cnt_words + P + 1 + edge_words) * 4));   // counts per (partition, chunk) | partition bases | edges
+        uint32_t* cnt = c->boff.as<uint32_t>();
+        uint32_t* pbase = cnt + cnt_words;
+        uint32_t* edge = pbase + P + 1;
+        // the spill area of partitions whose survivors exceed the shared-memory stage; the member records use it later
+        CU(c->rec_a.ensure((size_t)n * sizeof(IndelRec)));
         if (c->ticket_next >= (int)LB_ORDINALS) return set_err(CSV_E_STATE, "ticket pool exhausted");
-        BigBuckets BB{c->big_bkt.as<uint4>(), bb_cap, c->tickets.as<uint32_t>() + c->ticket_next++};
-        {
-            int g = (int)std::min<uint32_t>(n_tiles, (uint32_t)c->n_sm * 8);
-            if (c->ticket_next >= (int)LB_ORDINALS) return set_err(CSV_E_STATE, "ticket pool exhausted");
-            uint32_t* done_ctr = c->tickets.as<uint32_t>() + c->ticket_next++;
-#define BP_LAUNCH(RB) g = std::min(g, resident_grid(c, k_bucket_prefix<RB>, 256, 0)); LAUNCH_PDL(c, (k_bucket_prefix<RB>), g, 256, 0, c->bkt.as<uint32_t>(), n_buckets, rb, (uint32_t)J.cp.min_support, bpre, tile_base, BB, &ctr->status, done_ctr, n_pass)
-            switch (rb) {
-                case 1: BP_LAUNCH(1); break; case 2: BP_LAUNCH(2); break; case 3: BP_LAUNCH(3); break; case 4: BP_LAUNCH(4); break;
-                case 5: BP_LAUNCH(5); break; case 6: BP_LAUNCH(6); break; case 7: BP_LAUNCH(7); break; case 8: BP_LAUNCH(8); break;
-                default: BP_LAUNCH(0); break;
-            }
-#undef BP_LAUNCH
-        }
+        uint32_t* done_ctr = c->tickets.as<uint32_t>() + c->ticket_next++;
+        CU(cudaMemsetAsync(edge, 0, edge_words * 4, c->stream));
+        const int is_ins = t == CSV_INS ? 1 : 0;
+        LAUNCH(c, k_part_count, n_chunks, 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), n, is_ins, ct, W, P, n_chunks, rb, cnt, edge,
+               &ctr->status);
+        LAUNCH_PDL(c, k_part_scan, P, 256, 0, cnt, n_chunks, P, pbase, done_ctr);
         uint2* pairs = (uint2*)c->keys_a.p;   // 8 B per signature (ensure_lane_scratch)
-        LAUNCH_PDL(c, k_indel_scatter, grid_for(c, n, 256 * 4), 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), n, t == CSV_INS ? 1 : 0, ct,
-               (const uint32_t*)bpre, (const uint32_t*)tile_base, c->bkt.as<uint32_t>(), pairs);
+        LAUNCH_PDL(c, k_part_scatter, n_chunks, 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), n, is_ins, ct, W, P, n_chunks,
+                   (const uint32_t*)cnt, (const uint32_t*)pbase, pairs);
         stage_end(c, CSV_ST_KEYS);
         stage_begin(c, CSV_ST_SORT);
-        LAUNCH_PDL(c, k_bucket_fixup, grid_for(c, n, FX_TILE, 8), 256, 0, (const uint2*)pairs, n_pass, c->keys_b.as<uint32_t>(),
-               c->vals_b.as<uint32_t>(), c->bkt.as<uint32_t>(), (int64_t)n_bkt, BB, (const uint32_t*)tile_base);
+        TileSync ts;
+        rc = make_sync(c, (size_t)P, &ts);
+        if (rc) return rc;
+        uint32_t* n_pass = &ctr->n_dom[t];
+        const size_t smem = pf_smem_bytes(W);
+        const int g = std::min(P, resident_grid(c, k_part_filter, 256, smem));
+        LAUNCH_PDL(c, k_part_filter, g, 256, smem, (const uint2*)pairs, (const uint32_t*)pbase, P, W, rb, (uint32_t)J.cp.min_support,
+                   (const uint32_t*)edge, c->keys_b.as<uint32_t>(), c->vals_b.as<uint32_t>(), (uint2*)c->rec_a.p, n_pass, ts);
         stage_end(c, CSV_ST_SORT);
         J.n_dev = n_pass;
         J.keys32 = c->keys_b.as<uint32_t>();
         sidx = c->vals_b.as<uint32_t>();
     } else {
     stage_begin(c, CSV_ST_KEYS);
-    if (prefilter) {
-        // the bucket histogram is all-zero between calls: zeroed when (re)allocated, cleared again by k_prefilter
-        CU(c->bkt.ensure(n_bkt * 4, true));
-        CU(c->hist.ensure(RS_MAX_PASSES * 256 * 4));
-        const int passes = std::max(1, (bits + 7) / 8);
-        LAUNCH(c, (k_indel_keys<uint32_t, true>), grid_for(c, n, 256), 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), s.b.as<int32_t>(),
-               s.rid.as<int32_t>(), n, t == CSV_INS ? 1 : 0, ct, c->keys_b.as<uint32_t>(), &ctr->status, c->bkt.as<uint32_t>());
-        uint32_t* n_pass = &ctr->n_dom[t];
-        const uint32_t n_buckets = (uint32_t)(total >> BKT_SHIFT) + 1;
-        CU(c->bkt_flags.ensure(((size_t)n_buckets / 32 + 2) * 4));
-        LAUNCH(c, k_bucket_flags, grid_for(c, n_buckets / 16 + 256, 256, 8), 256, 0, c->bkt.as<uint32_t>(), n_buckets, rb, (uint32_t)J.cp.min_support,
-               c->bkt_flags.as<uint32_t>(), c->hist.as<uint32_t>(), RS_MAX_PASSES * 256);
-        LAUNCH(c, k_prefilter, grid_for(c, n, 2048, 8), 256, 0, c->keys_b.as<uint32_t>(), n, c->bkt_flags.as<uint32_t>(),
-               c->keys_a.as<uint32_t>(), c->vals_a.as<uint32_t>(), n_pass, c->bkt.as<uint32_t>(), (int64_t)n_bkt, c->hist.as<uint32_t>(),
-               passes);
-        J.n_dev = n_pass;
-    } else if (!k64)
-        LAUNCH(c, (k_indel_keys<uint32_t, false>), grid_for(c, n, 256), 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), s.b.as<int32_t>(),
-               s.rid.as<int32_t>(), n, t == CSV_INS ? 1 : 0, ct, c->keys_a.as<uint32_t>(), &ctr->status, (uint32_t*)nullptr);
+    if (!k64)
+        LAUNCH(c, (k_indel_keys<uint32_t>), grid_for(c, n, 256), 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), s.b.as<int32_t>(),
+               s.rid.as<int32_t>(), n, t == CSV_INS ? 1 : 0, ct, c->keys_a.as<uint32_t>(), &ctr->status);
     else
-        LAUNCH(c, (k_indel_keys<uint64_t, false>), grid_for(c, n, 256), 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), s.b.as<int32_t>(),
-               s.rid.as<int32_t>(), n, t == CSV_INS ? 1 : 0, ct, c->keys_a.as<uint64_t>(), &ctr->status, (uint32_t*)nullptr);
+        LAUNCH(c, (k_indel_keys<uint64_t>), grid_for(c, n, 256), 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), s.b.as<int32_t>(),
+               s.rid.as<int32_t>(), n, t == CSV_INS ? 1 : 0, ct, c->keys_a.as<uint64_t>(), &ctr->status);
     stage_end(c, CSV_ST_KEYS);
     stage_begin(c, CSV_ST_SORT);
     if (!k64) {
         uint32_t* ko = nullptr;
         rc = radix_sort<uint32_t>(c, c->keys_a.as<uint32_t>(), c->vals_a.as<uint32_t>(), c->keys_b.as<uint32_t>(),
-                                  c->vals_b.as<uint32_t>(), !prefilter, n, J.n_dev, bits, &ko, &sidx, t, prefilter);
+                                  c->vals_b.as<uint32_t>(), true, n, nullptr, bits, &ko, &sidx);
         J.keys32 = ko;
     } else {
         uint64_t* ko = nullptr;
@@ -1031,7 +1005,7 @@ static int run_indel(csv_ctx* c, int t, uint32_t kslot_base) {
     }
     J.iv.is_ins = t == CSV_INS ? 1 : 0;
     J.small_path = c->small_path_enabled ? 1 : 0;
-    c->prev_is_chain_kernel = bucket_sort;
+    c->prev_is_chain_kernel = prefilter;
     rc = run_segment_and_cluster(c, J, t, kslot_base);
     c->prev_is_chain_kernel = false;
     return rc;
@@ -1115,10 +1089,10 @@ static int run_other(csv_ctx* c, int t, uint32_t kslot_base) {
 static void lane_swap(csv_ctx* c, LaneWork& L) {
     std::swap(c->stream, L.stream);
     std::swap(c->keys_a, L.keys_a); std::swap(c->keys_b, L.keys_b); std::swap(c->vals_a, L.vals_a); std::swap(c->vals_b, L.vals_b);
-    std::swap(c->hist, L.hist); std::swap(c->lb_status, L.lb_status); std::swap(c->bkt, L.bkt); std::swap(c->bkt_flags, L.bkt_flags);
+    std::swap(c->hist, L.hist); std::swap(c->lb_status, L.lb_status);
     std::swap(c->big_list, L.big_list); std::swap(c->giant_list, L.giant_list); std::swap(c->giant_arena, L.giant_arena);
     std::swap(c->boff, L.boff); std::swap(c->rec_a, L.rec_a); std::swap(c->rec_b, L.rec_b); std::swap(c->recc_a, L.recc_a);
-    std::swap(c->recc_b, L.recc_b); std::swap(c->big_bkt, L.big_bkt); std::swap(c->rest_list, L.rest_list);
+    std::swap(c->recc_b, L.recc_b); std::swap(c->rest_list, L.rest_list);
     std::swap(c->small, L.small);
 }
 static int ensure_small(csv_ctx* c, size_t ns) {

@@ -256,10 +256,10 @@ __global__ void __launch_bounds__(256) k_expand_contigs(const int64_t* __restric
 
 // Four consecutive signatures per thread and iteration through 128-bit loads (64 B of loads in flight per
 // thread: the kernel is a latency-bound stream); a scalar loop takes the tail / unaligned columns.
-template <typename K, bool HIST>
+template <typename K>
 __global__ void __launch_bounds__(256) k_indel_keys(const int32_t* __restrict__ chrom, const int32_t* __restrict__ a, const int32_t* __restrict__ b,
                              const int32_t* __restrict__ rid, int64_t n, int is_ins, ContigTab ct, K* __restrict__ keys,
-                             uint32_t* status, uint32_t* __restrict__ bkt) {
+                             uint32_t* status) {
     auto one = [&](int32_t c, int32_t raw, int32_t bb, int32_t rr, uint32_t& bad) -> K {
         K key = 0;
         if (c < 0 || c >= ct.n) bad |= ST_BAD_CHROM;
@@ -285,124 +285,13 @@ __global__ void __launch_bounds__(256) k_indel_keys(const int32_t* __restrict__ 
             reinterpret_cast<ulonglong2*>(keys)[2 * v] = make_ulonglong2((uint64_t)k0, (uint64_t)k1);
             reinterpret_cast<ulonglong2*>(keys)[2 * v + 1] = make_ulonglong2((uint64_t)k2, (uint64_t)k3);
         }
-        if (HIST) {
-            atomicAdd(&bkt[(uint32_t)(k0 >> BKT_SHIFT) + BKT_PAD], 1u); atomicAdd(&bkt[(uint32_t)(k1 >> BKT_SHIFT) + BKT_PAD], 1u);
-            atomicAdd(&bkt[(uint32_t)(k2 >> BKT_SHIFT) + BKT_PAD], 1u); atomicAdd(&bkt[(uint32_t)(k3 >> BKT_SHIFT) + BKT_PAD], 1u);
-        }
     }
     for (int64_t i = nv * 4 + tid; i < n; i += stride) {
         const K key = one(chrom[i], a[i], b[i], rid[i], bad);
         keys[i] = key;
-        if (HIST) atomicAdd(&bkt[(uint32_t)(key >> BKT_SHIFT) + BKT_PAD], 1u);
     }
     if (bad) atomicOr(status, bad);
 }
-
-// pass 2 of the density filter: one bit per bucket = "the +-rb bucket neighbourhood holds >= need
-// signatures" (a superset of the +-R window of every signature in the bucket).  The bit map is
-// 1.5 MB for hg19 and stays cache resident for the per-signature test.
-__global__ void __launch_bounds__(256) k_bucket_flags(const uint32_t* __restrict__ bkt, uint32_t n_buckets, int rb, uint32_t need,
-                                                      uint32_t* __restrict__ flags, uint32_t* __restrict__ hist_to_clear, int hist_words) {
-    if (blockIdx.x == 0)   // the radix digit histograms k_prefilter accumulates into
-        for (int i = threadIdx.x; i < hist_words; i += 256) hist_to_clear[i] = 0u;
-    // A CTA stages 4096 buckets (+ halo) in shared memory with coalesced loads; every thread then
-    // slides the window sum along its 16 consecutive buckets; lane pairs assemble a 32-bit word.
-    constexpr int PER = 16, TILE = 256 * PER;
-    __shared__ uint32_t s_b[(TILE + 2 * BKT_PAD + 8) * 17 / 16 + 8];
-    auto P = [](int i) { return i + (i >> 4); };  // +1 word per 16: threads stride 17 words -> no bank conflicts
-    const uint32_t n_tiles = (n_buckets + TILE - 1) / TILE;
-    for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        const int64_t t0 = (int64_t)tile * TILE;                 // first bucket of the tile
-        // s_b[i] = bkt[t0 - rb + i + PAD], i in [0, TILE + 2*rb + 1)
-        for (int i = threadIdx.x; i < TILE + 2 * rb + 1; i += 256) s_b[P(i)] = bkt[t0 - rb + i + BKT_PAD];
-        __syncthreads();
-        const int l0 = threadIdx.x * PER;                        // local index of the thread's first bucket
-        uint32_t sum = 0, mask = 0;
-        for (int k = 0; k <= 2 * rb; k++) sum += s_b[P(l0 + k)];
-#pragma unroll
-        for (int j = 0; j < PER; j++) {
-            if (t0 + l0 + j < n_buckets && sum >= need) mask |= 1u << j;
-            sum += s_b[P(l0 + j + 2 * rb + 1)] - s_b[P(l0 + j)];
-        }
-        const uint32_t other = __shfl_down_sync(0xffffffffu, mask, 1);
-        const int64_t word = (t0 + l0) >> 5;
-        if ((threadIdx.x & 1) == 0 && t0 + l0 < n_buckets) flags[word] = mask | (other << 16);
-        __syncthreads();
-    }
-}
-
-// survivors of the density filter, compacted (order irrelevant: every later tie-break uses the
-// original input index).  2048 signatures per CTA iteration, one reservation atomic per iteration.
-__global__ void __launch_bounds__(256) k_prefilter(const uint32_t* __restrict__ keys, int64_t n, const uint32_t* __restrict__ flags,
-                                                   uint32_t* __restrict__ out_keys, uint32_t* __restrict__ out_idx,
-                                                   uint32_t* out_count, uint32_t* __restrict__ bkt, int64_t n_bkt,
-                                                   uint32_t* __restrict__ hist, int passes) {
-    constexpr int ITEMS = 8;
-    __shared__ uint32_t s_warp[10];
-    __shared__ uint32_t s_hist[RS_MAX_PASSES * 256];
-    // Two chores ride along: the bucket histogram is cleared for the next call (it was consumed by k_bucket_flags; the
-    // buffer is all-zero between calls), and the survivors' digit histograms of every radix pass are accumulated here
-    // instead of in a separate read of the compacted keys (hist was zeroed by k_bucket_flags).
-    for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < n_bkt; i += (int64_t)gridDim.x * 256) bkt[i] = 0u;
-    for (int i = threadIdx.x; i < passes * 256; i += 256) s_hist[i] = 0;
-    __syncthreads();
-    const int64_t n_tiles = (n + 256 * ITEMS - 1) / (256 * ITEMS);
-    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        const int64_t base = tile * 256 * ITEMS;
-        uint32_t key[ITEMS];
-        uint32_t passm = 0, cnt = 0;
-#pragma unroll
-        for (int j = 0; j < ITEMS; j++) {
-            const int64_t i = base + j * 256 + threadIdx.x;
-            key[j] = i < n ? keys[i] : 0u;
-        }
-#pragma unroll
-        for (int j = 0; j < ITEMS; j++) {
-            const int64_t i = base + j * 256 + threadIdx.x;
-            const uint32_t b = key[j] >> BKT_SHIFT;
-            const bool pass = i < n && ((__ldg(&flags[b >> 5]) >> (b & 31)) & 1u);
-            if (pass) { passm |= 1u << j; cnt++; }
-        }
-        uint32_t o = block_reserve_256(cnt, out_count, s_warp);
-#pragma unroll
-        for (int j = 0; j < ITEMS; j++) {
-            if (passm >> j & 1u) {
-                out_keys[o] = key[j];
-                out_idx[o] = (uint32_t)(base + j * 256 + threadIdx.x);
-                o++;
-                for (int p = 0; p < passes; p++) atomicAdd(&s_hist[p * 256 + (int)((key[j] >> (8 * p)) & 0xff)], 1u);
-            }
-        }
-    }
-    __syncthreads();
-    for (int i = threadIdx.x; i < passes * 256; i += 256) {
-        const uint32_t v = s_hist[i];
-        if (v) atomicAdd(&hist[i], v);
-    }
-}
-
-// ------------------------------------------------------------------------------------------
-// INS / DEL front end, filter-first: "density filter -> bucket counting sort -> in-bucket order -> member records"
-// (replaces: keys pass + compaction + four stable radix passes over (key, index) + the member gathers of the
-//  cluster kernels).  The bucket histogram the filter needs anyway IS a counting-sort histogram: a prefix sum over
-//  the counts of the flagged buckets gives every flagged bucket its slot range, so ONE scatter pass puts every
-//  survivor into bucket order and a tile-local pass orders the few signatures inside each 256-bp bucket.  The order
-//  among equal keys is irrelevant: every later tie-break uses the input index.
-//  While the bucket tables stay in L2 (the host only takes this path then), what bounds these kernels is not DRAM bytes
-//  but the rate of UNCOALESCED 4-8 B accesses (one L1 wavefront each): the design minimises those -- per signature one RED and one table look-up, per
-//  survivor one returning atomic and one 8 B store, per member of a kept cluster one record gather.
-//    k_indel_hist      8 B/sig read (chrom, a)                 + one RED per signature
-//    k_bucket_prefix   4 B/bucket read, 4 B/bucket written     flag + slot offset inside the 4096-bucket tile
-//    k_scan_small      tile totals -> tile bases               (a few thousand words, one CTA)
-//    k_indel_scatter   8 B/sig read + one look-up              -> (key, index) 8 B per survivor, bucket order
-//    k_bucket_fixup    8 B/survivor read + written             in-bucket order (+ clears the histogram)
-//    k_select_heads    4 B/survivor read (chain votes)         -> 16-20 B record per member of a kept cluster
-// ------------------------------------------------------------------------------------------
-static constexpr int FIX_SMALL = 64;                    // buckets with more survivors than this are ordered by a CTA (k_bucket_fixup_big)
-static constexpr int BP_PER = 16, BP_TILE = 256 * BP_PER;   // buckets per tile of k_bucket_prefix
-static constexpr int BP_TILE_SHIFT = 12;
-static_assert((1 << BP_TILE_SHIFT) == BP_TILE, "tile size");
-static constexpr uint32_t BP_NONE = 0xffffffffu;        // bpre[] of a bucket that is not flagged
 
 __device__ __forceinline__ uint32_t indel_key32(int32_t c, int32_t raw, int is_ins, const ContigTab& ct, uint32_t& bad) {
     if (c < 0 || c >= ct.n) { bad |= ST_BAD_CHROM; return 0u; }
@@ -411,263 +300,340 @@ __device__ __forceinline__ uint32_t indel_key32(int32_t c, int32_t raw, int is_i
     return (uint32_t)(ct.off[c] + (uint64_t)pos);
 }
 
-__global__ void __launch_bounds__(256) k_indel_hist(const int32_t* __restrict__ chrom, const int32_t* __restrict__ a, int64_t n, int is_ins,
-                                                    ContigTab ct, uint32_t* status, uint32_t* __restrict__ bkt) {
-    pdl_launch_dependents();   // the next kernel of the chain may become resident now (it waits for this grid to finish)
-    const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (int64_t)gridDim.x * blockDim.x;
-    const bool aligned = ((((uintptr_t)chrom) | ((uintptr_t)a)) & 15) == 0;
-    const int64_t nv = aligned ? (n >> 2) : 0;
-    uint32_t bad = 0;
-    for (int64_t v = tid; v < nv; v += stride) {
-        const int4 c4 = __ldcs(reinterpret_cast<const int4*>(chrom) + v), a4 = __ldcs(reinterpret_cast<const int4*>(a) + v);
-        const uint32_t k0 = indel_key32(c4.x, a4.x, is_ins, ct, bad), k1 = indel_key32(c4.y, a4.y, is_ins, ct, bad);
-        const uint32_t k2 = indel_key32(c4.z, a4.z, is_ins, ct, bad), k3 = indel_key32(c4.w, a4.w, is_ins, ct, bad);
-        atomicAdd(&bkt[(k0 >> BKT_SHIFT) + BKT_PAD], 1u); atomicAdd(&bkt[(k1 >> BKT_SHIFT) + BKT_PAD], 1u);
-        atomicAdd(&bkt[(k2 >> BKT_SHIFT) + BKT_PAD], 1u); atomicAdd(&bkt[(k3 >> BKT_SHIFT) + BKT_PAD], 1u);
-    }
-    for (int64_t i = nv * 4 + tid; i < n; i += stride) atomicAdd(&bkt[(indel_key32(chrom[i], a[i], is_ins, ct, bad) >> BKT_SHIFT) + BKT_PAD], 1u);
-    if (bad) atomicOr(status, bad);
+// ------------------------------------------------------------------------------------------
+// INS / DEL front end, partitioned: the genome's linear coordinate is cut into P partitions of 2^W bp (W <= 22, so a
+// partition has at most 16384 buckets of 256 bp).  The density filter then needs no genome-sized bucket table: every
+// partition's histogram is built, flagged, scanned and used inside one CTA's shared memory.
+//    k_part_count    8 B/sig read (chrom, a)          -> (partition, chunk) counts; halo counts at partition edges
+//    k_part_scan     4 B per (partition, chunk)       -> slot of every chunk inside every partition
+//    k_part_scatter  8 B/sig read, 8 B/sig written    -> (key, index) pairs grouped by partition
+//    k_part_filter   8 B/sig read (twice, the second  -> survivors in key order, 8 B per survivor written
+//                    mostly from L2)
+// ------------------------------------------------------------------------------------------
+static constexpr int PART_CHUNK = 16384;     // signatures per CTA of k_part_count / k_part_scatter
+static constexpr int PART_MAX = 1024;        // partitions: 32-bit keys, W = 22
+static constexpr int PART_W_MAX = 22;
+static constexpr int PART_W_MIN = 16;        // >= 256 buckets per partition: the +-BKT_PAD halo reaches the neighbours only
+static constexpr int PF_STAGE = 5632;        // survivors of one partition ordered in shared memory; more spill to global
+static constexpr int FIX_SMALL = 64;         // buckets with more survivors than this are ordered by a counting sort
+static constexpr int PF_BIG_CAP = 256;       // buckets of more than FIX_SMALL survivors listed per partition
+__host__ __device__ constexpr size_t pf_smem_bytes(int w) {
+    return (size_t)(1u << (w - BKT_SHIFT)) * 4 + (size_t)(1u << (w - BKT_SHIFT)) / 32 * 4 + (size_t)PF_STAGE * 8;
 }
 
-// per bucket: bpre[b] = number of survivors in flagged buckets before b INSIDE its tile, or BP_NONE when the +-rb
-// bucket neighbourhood holds fewer than `need` signatures; tile_tot[tile] = survivors of the tile.  Buckets with
-// more than FIX_SMALL survivors are listed for the CTA-sized in-bucket pass.  Every tile is independent (no
-// look-back chain): one streaming read of the histogram, one streaming write of bpre.
-struct BigBuckets { uint4* list; uint32_t cap; uint32_t* count; };   // (tile, offset inside the tile, count, -)
-// RB in 1..8: neighbourhood radius known at compile time, every thread keeps its 16 buckets + halo (32 counts, eight
-// 128-bit loads) in registers; RB == 0: any radius <= BKT_PAD through a shared-memory tile.
-template <int RB>
-__global__ void __launch_bounds__(256) k_bucket_prefix(const uint32_t* __restrict__ bkt, uint32_t n_buckets, int rb, uint32_t need,
-                                                       uint32_t* __restrict__ bpre, uint32_t* __restrict__ tile_tot, BigBuckets BB,
-                                                       uint32_t* status, uint32_t* done_ctr, uint32_t* n_out) {
-    pdl_launch_dependents(); pdl_wait();   // programmatic dependent launch: resident early, starts when the previous kernel has finished
-    __shared__ uint32_t s_b[RB == 0 ? (BP_TILE + 2 * BKT_PAD + 8) * 17 / 16 + 8 : 1];
+// One chunk of PART_CHUNK rows per CTA: f(key, row) for every row, with the same validation as k_indel_keys.
+template <class F>
+__device__ __forceinline__ void part_rows(const int32_t* __restrict__ chrom, const int32_t* __restrict__ a, int64_t n, int is_ins,
+                                          const ContigTab& ct, uint32_t& bad, F f) {
+    const int64_t c0 = (int64_t)blockIdx.x * PART_CHUNK;
+    const int64_t c1 = min(c0 + (int64_t)PART_CHUNK, n);
+    const bool aligned = ((((uintptr_t)chrom) | ((uintptr_t)a)) & 15) == 0;
+    const int64_t v1 = aligned ? (c1 >> 2) : (c0 >> 2);   // c0 is a multiple of 4
+    for (int64_t v = (c0 >> 2) + threadIdx.x; v < v1; v += blockDim.x) {
+        const int4 c4 = __ldcs(reinterpret_cast<const int4*>(chrom) + v), a4 = __ldcs(reinterpret_cast<const int4*>(a) + v);
+        f(indel_key32(c4.x, a4.x, is_ins, ct, bad), 4 * v);
+        f(indel_key32(c4.y, a4.y, is_ins, ct, bad), 4 * v + 1);
+        f(indel_key32(c4.z, a4.z, is_ins, ct, bad), 4 * v + 2);
+        f(indel_key32(c4.w, a4.w, is_ins, ct, bad), 4 * v + 3);
+    }
+    for (int64_t i = v1 * 4 + threadIdx.x; i < c1; i += blockDim.x) f(indel_key32(chrom[i], a[i], is_ins, ct, bad), i);
+}
+
+// cnt[p * n_chunks + chunk] = rows of the chunk in partition p.  edge[p][j] (j < BKT_PAD) counts the rows in the j-th
+// bucket of partition p, edge[p][BKT_PAD + j] those in its j-th bucket from the end: the halo of the neighbours' windows.
+__global__ void __launch_bounds__(256) k_part_count(const int32_t* __restrict__ chrom, const int32_t* __restrict__ a, int64_t n, int is_ins,
+                                                    ContigTab ct, int W, int P, int n_chunks, int rb, uint32_t* __restrict__ cnt,
+                                                    uint32_t* __restrict__ edge, uint32_t* status) {
+    pdl_launch_dependents();
+    __shared__ uint32_t s_c[PART_MAX];
+    for (int p = threadIdx.x; p < P; p += blockDim.x) s_c[p] = 0;
+    __syncthreads();
+    const uint32_t bmask = (1u << (W - BKT_SHIFT)) - 1;
+    uint32_t bad = 0;
+    part_rows(chrom, a, n, is_ins, ct, bad, [&](uint32_t key, int64_t) {
+        const uint32_t p = key >> W, bl = (key >> BKT_SHIFT) & bmask;
+        atomicAdd(&s_c[p], 1u);
+        if (bl < (uint32_t)rb) atomicAdd(&edge[p * 2 * BKT_PAD + bl], 1u);
+        if (bmask - bl < (uint32_t)rb) atomicAdd(&edge[p * 2 * BKT_PAD + BKT_PAD + (bmask - bl)], 1u);
+    });
+    if (bad) atomicOr(status, bad);
+    __syncthreads();
+    for (int p = threadIdx.x; p < P; p += blockDim.x) cnt[(int64_t)p * n_chunks + blockIdx.x] = s_c[p];
+}
+
+// One CTA per partition: its row of cnt becomes exclusive offsets inside the partition; the CTA that finishes last turns
+// the partition totals into partition bases: base[p] = first pair of partition p, base[P] = n.
+__global__ void __launch_bounds__(256) k_part_scan(uint32_t* __restrict__ cnt, int n_chunks, int P, uint32_t* __restrict__ base,
+                                                   uint32_t* done_ctr) {
+    pdl_launch_dependents(); pdl_wait();
     __shared__ uint32_t s_warp[9];
     __shared__ uint32_t s_last;
-    auto P = [](int i) { return i + (i >> 4); };   // +1 word per 16: threads stride 17 words -> no bank conflicts
-    const uint32_t n_tiles = (n_buckets + BP_TILE - 1) / BP_TILE;
-    for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        const int64_t t0 = (int64_t)tile * BP_TILE;
-        const int l0 = threadIdx.x * BP_PER;
-        uint32_t mask = 0, mine = 0;
-        uint32_t own[BP_PER];
-        if (RB > 0) {
-            // w[k] = count of bucket t0 + l0 - 8 + k; (BKT_PAD - 8) words keep the 16 B alignment
-            uint32_t w[32];
-            const uint4* src = reinterpret_cast<const uint4*>(bkt + BKT_PAD + t0 + l0 - 8);
-#pragma unroll
-            for (int k = 0; k < 8; k++) { const uint4 x = __ldg(src + k); w[4 * k] = x.x; w[4 * k + 1] = x.y; w[4 * k + 2] = x.z; w[4 * k + 3] = x.w; }
-            uint32_t sum = 0;
-#pragma unroll
-            for (int k = 8 - RB; k <= 8 + RB; k++) sum += w[k];
-#pragma unroll
-            for (int j = 0; j < BP_PER; j++) {
-                own[j] = w[8 + j];
-                if (t0 + l0 + j < n_buckets && sum >= need) { mask |= 1u << j; mine += own[j]; }
-                if (j + 1 < BP_PER) sum += w[8 + j + RB + 1] - w[8 + j - RB];
-            }
-        } else {
-            for (int i = threadIdx.x; i < BP_TILE + 2 * rb + 1; i += 256) s_b[P(i)] = bkt[t0 - rb + i + BKT_PAD];
-            __syncthreads();
-            uint32_t sum = 0;
-            for (int k = 0; k <= 2 * rb; k++) sum += s_b[P(l0 + k)];
-#pragma unroll
-            for (int j = 0; j < BP_PER; j++) {
-                own[j] = s_b[P(l0 + j + rb)];
-                if (t0 + l0 + j < n_buckets && sum >= need) { mask |= 1u << j; mine += own[j]; }
-                sum += s_b[P(l0 + j + 2 * rb + 1)] - s_b[P(l0 + j)];
-            }
-        }
+    uint32_t* row = cnt + (int64_t)blockIdx.x * n_chunks;
+    uint32_t carry = 0;
+    for (int b = 0; b < n_chunks; b += 256) {
+        const int i = b + threadIdx.x;
+        const uint32_t v = i < n_chunks ? row[i] : 0u;
         uint32_t total;
-        uint32_t run = block_excl_scan_256(mine, s_warp, &total);
-        if (threadIdx.x == 0) tile_tot[tile] = total;
-        uint32_t o[BP_PER];
-#pragma unroll
-        for (int j = 0; j < BP_PER; j++) {
-            o[j] = BP_NONE;
-            if (mask >> j & 1u) {
-                const uint32_t cnt = own[j];
-                o[j] = run;
-                if (cnt > FIX_SMALL) {
-                    const uint32_t q = atomicAdd(BB.count, 1u);
-                    if (q < BB.cap) BB.list[q] = make_uint4(tile, run, cnt, 0u); else atomicOr(status, ST_LIST_OVERFLOW);
-                }
-                run += cnt;
-            }
-        }
-        uint4* dst = reinterpret_cast<uint4*>(bpre + t0 + l0);   // bpre is sized to whole tiles
-#pragma unroll
-        for (int j = 0; j < BP_PER; j += 4) dst[j >> 2] = make_uint4(o[j], o[j + 1], o[j + 2], o[j + 3]);
-        if (RB == 0) __syncthreads();
+        const uint32_t ex = block_excl_scan_256(v, s_warp, &total);
+        if (i < n_chunks) row[i] = carry + ex;
+        carry += total;
     }
-    // the CTA that finishes last turns the tile totals into tile bases (a few thousand words) and reports the number of
-    // survivors: no separate scan launch
+    if (threadIdx.x == 0) base[blockIdx.x] = carry;
     __threadfence();
     if (threadIdx.x == 0) s_last = atomicAdd(done_ctr, 1u) == gridDim.x - 1 ? 1u : 0u;
     __syncthreads();
     if (!s_last) return;
     __threadfence();
-    uint32_t carry = 0;
-    for (uint32_t base = 0; base < n_tiles; base += 256) {
-        const uint32_t i = base + threadIdx.x;
-        const uint32_t v = i < n_tiles ? __ldcg(&tile_tot[i]) : 0u;
+    carry = 0;
+    for (int b = 0; b < P; b += 256) {
+        const int i = b + threadIdx.x;
+        const uint32_t v = i < P ? __ldcg(&base[i]) : 0u;
         uint32_t total;
         const uint32_t ex = block_excl_scan_256(v, s_warp, &total);
-        if (i < n_tiles) tile_tot[i] = carry + ex;
+        if (i < P) base[i] = carry + ex;
         carry += total;
     }
-    if (threadIdx.x == 0) *n_out = carry;
+    if (threadIdx.x == 0) base[P] = carry;
 }
 
-// exclusive scan of arr[0..n) by ONE CTA (n: a few thousand words), *total_out = sum
-__global__ void __launch_bounds__(1024) k_scan_small(uint32_t* arr, int64_t n, uint32_t* total_out) {
-    __shared__ uint32_t s_w[33];
-    __shared__ uint32_t s_run;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) s_run = 0;
-    __syncthreads();
-    for (int64_t base = 0; base < n; base += 1024) {
-        const int64_t i = base + threadIdx.x;
-        const uint32_t v = i < n ? arr[i] : 0u;
-        uint32_t incl = v;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += y; }
-        if (lane == 31) s_w[warp] = incl;
-        __syncthreads();
-        if (warp == 0) {
-            const uint32_t w = s_w[lane];
-            uint32_t wi = w;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, wi, d); if (lane >= d) wi += y; }
-            s_w[lane] = wi - w;
-            if (lane == 31) s_w[32] = wi;
-        }
-        __syncthreads();
-        if (i < n) arr[i] = s_run + s_w[warp] + incl - v;
-        __syncthreads();
-        if (threadIdx.x == 0) s_run += s_w[32];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0 && total_out) *total_out = s_run;
-}
-
-// survivors into bucket order: slot = tile base + offset of the bucket inside its tile + (count of the bucket,
-// counted down by one returning atomic).  Afterwards every flagged bucket's count is zero again.
-// (Tried: counting the slots up in bpre[] itself, so that the atomic lands on the sector the look-up has just brought
-//  into L2 and the histogram is not touched again -- 48 MB less DRAM traffic per launch, but 3 % slower: the atomics
-//  then share sectors with the 8.4 M look-ups still in flight.)
-__global__ void __launch_bounds__(256) k_indel_scatter(const int32_t* __restrict__ chrom, const int32_t* __restrict__ a, int64_t n, int is_ins,
-                                                       ContigTab ct, const uint32_t* __restrict__ bpre, const uint32_t* __restrict__ tile_base,
-                                                       uint32_t* __restrict__ bkt, uint2* __restrict__ pairs_out) {
-    pdl_launch_dependents(); pdl_wait();   // programmatic dependent launch: resident early, starts when the previous kernel has finished
-    const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (int64_t)gridDim.x * blockDim.x;
-    const bool aligned = ((((uintptr_t)chrom) | ((uintptr_t)a)) & 15) == 0;
-    const int64_t nv = aligned ? (n >> 2) : 0;
-    uint32_t dummy = 0;   // validated by k_indel_hist
-    auto place = [&](uint32_t key, uint32_t pre, int64_t i) {
-        const uint32_t bu = key >> BKT_SHIFT;
-        const uint32_t old = atomicSub(&bkt[bu + BKT_PAD], 1u);
-        pairs_out[__ldg(&tile_base[bu >> BP_TILE_SHIFT]) + pre + old - 1u] = make_uint2(key, (uint32_t)i);
-    };
-    for (int64_t v = tid; v < nv; v += stride) {
-        const int4 c4 = __ldcs(reinterpret_cast<const int4*>(chrom) + v), a4 = __ldcs(reinterpret_cast<const int4*>(a) + v);
-        const uint32_t k0 = indel_key32(c4.x, a4.x, is_ins, ct, dummy), k1 = indel_key32(c4.y, a4.y, is_ins, ct, dummy);
-        const uint32_t k2 = indel_key32(c4.z, a4.z, is_ins, ct, dummy), k3 = indel_key32(c4.w, a4.w, is_ins, ct, dummy);
-        // the four look-ups are independent: all in flight before the first is used
-        const uint32_t p0 = __ldg(&bpre[k0 >> BKT_SHIFT]), p1 = __ldg(&bpre[k1 >> BKT_SHIFT]);
-        const uint32_t p2 = __ldg(&bpre[k2 >> BKT_SHIFT]), p3 = __ldg(&bpre[k3 >> BKT_SHIFT]);
-        if (p0 != BP_NONE) place(k0, p0, 4 * v);
-        if (p1 != BP_NONE) place(k1, p1, 4 * v + 1);
-        if (p2 != BP_NONE) place(k2, p2, 4 * v + 2);
-        if (p3 != BP_NONE) place(k3, p3, 4 * v + 3);
-    }
-    for (int64_t i = nv * 4 + tid; i < n; i += stride) {
-        const uint32_t key = indel_key32(chrom[i], a[i], is_ins, ct, dummy);
-        const uint32_t pre = __ldg(&bpre[key >> BKT_SHIFT]);
-        if (pre != BP_NONE) place(key, pre, i);
-    }
-}
-
-// order inside every bucket: destination = bucket start + number of bucket members with a smaller (key, slot).
-// A CTA stages 2048 slots + a halo of FIX_SMALL on both sides in shared memory (coalesced), every thread ranks its
-// 8 slots against their buckets there.  Buckets of more than FIX_SMALL survivors: k_bucket_fixup_big.  Rides along:
-// the bucket histogram is cleared for the next call (flagged buckets were counted down to zero, the others not).
-static constexpr int FX_TILE = 2048;
-__global__ void __launch_bounds__(256) k_bucket_fixup(const uint2* __restrict__ pairs, const uint32_t* n_dev, uint32_t* __restrict__ keys_out,
-                                                      uint32_t* __restrict__ idx_out, uint32_t* __restrict__ bkt, int64_t n_bkt, BigBuckets BB,
-                                                      const uint32_t* __restrict__ tile_base) {
-    pdl_launch_dependents(); pdl_wait();   // programmatic dependent launch: resident early, starts when the previous kernel has finished
-    __shared__ uint32_t s_k[FX_TILE + 2 * FIX_SMALL];
+// (key, row) pairs grouped by partition; the order inside a partition is irrelevant (k_part_filter orders it).  The rows
+// of a chunk are grouped by partition in shared memory, PART_SUB at a time, so that every partition's run is written with
+// coalesced stores: single 8 B stores scattered over a buffer larger than L2 end up as partial-sector writes to DRAM.
+static constexpr int PART_SUB = 4096, PART_SUB_ITEMS = PART_SUB / 256;
+static_assert(PART_CHUNK % PART_SUB == 0 && PART_MAX == 4 * 256, "k_part_scatter tiling");
+__global__ void __launch_bounds__(256, 2) k_part_scatter(const int32_t* __restrict__ chrom, const int32_t* __restrict__ a, int64_t n, int is_ins,
+                                                      ContigTab ct, int W, int P, int n_chunks, const uint32_t* __restrict__ cnt,
+                                                      const uint32_t* __restrict__ base, uint2* __restrict__ pairs) {
+    pdl_launch_dependents(); pdl_wait();
+    __shared__ uint32_t s_cur[PART_MAX];   // next slot of every partition in `pairs`
+    __shared__ uint32_t s_off[PART_MAX];   // rows of the sub-tile per partition -> their first position in s_st
+    __shared__ uint2 s_st[PART_SUB];
     __shared__ uint32_t s_warp[9];
-    {
-        uint4* b4 = reinterpret_cast<uint4*>(bkt);   // n_bkt is a multiple of 4, cudaMalloc alignment
-        const uint4 z = make_uint4(0u, 0u, 0u, 0u);
-        for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < (n_bkt >> 2); i += (int64_t)gridDim.x * 256) b4[i] = z;
-    }
-    const int64_t n = *n_dev;
-    const int64_t n_tiles = (n + FX_TILE - 1) / FX_TILE;
-    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        const int64_t base = tile * FX_TILE;
-        for (int q = threadIdx.x; q < FX_TILE + 2 * FIX_SMALL; q += 256) {
-            const int64_t i = base - FIX_SMALL + q;
-            s_k[q] = (i >= 0 && i < n) ? pairs[i].x : 0u;
+    for (int p = threadIdx.x; p < P; p += blockDim.x) s_cur[p] = base[p] + cnt[(int64_t)p * n_chunks + blockIdx.x];
+    const int64_t c1 = min((int64_t)(blockIdx.x + 1) * PART_CHUNK, n);
+    uint32_t dummy = 0;   // validated by k_part_count
+    for (int64_t s0 = (int64_t)blockIdx.x * PART_CHUNK; s0 < c1; s0 += PART_SUB) {
+        const int m = (int)min((int64_t)PART_SUB, c1 - s0);
+        for (int p = threadIdx.x; p < PART_MAX; p += 256) s_off[p] = 0;
+        __syncthreads();
+        uint32_t key[PART_SUB_ITEMS], rank[PART_SUB_ITEMS];
+#pragma unroll
+        for (int j = 0; j < PART_SUB_ITEMS; j++) {
+            const int q = j * 256 + threadIdx.x;
+            key[j] = q < m ? indel_key32(chrom[s0 + q], a[s0 + q], is_ins, ct, dummy) : 0u;
+        }
+#pragma unroll
+        for (int j = 0; j < PART_SUB_ITEMS; j++)
+            if (j * 256 + (int)threadIdx.x < m) rank[j] = atomicAdd(&s_off[key[j] >> W], 1u);
+        __syncthreads();
+        {   // exclusive scan of the per-partition counts, four partitions per thread
+            const uint4 v = reinterpret_cast<const uint4*>(s_off)[threadIdx.x];
+            uint32_t total;
+            const uint32_t ex = block_excl_scan_256(v.x + v.y + v.z + v.w, s_warp, &total);
+            reinterpret_cast<uint4*>(s_off)[threadIdx.x] = make_uint4(ex, ex + v.x, ex + v.x + v.y, ex + v.x + v.y + v.z);
         }
         __syncthreads();
-#pragma unroll 2
-        for (int j = 0; j < FX_TILE / 256; j++) {
-            const int q = FIX_SMALL + j * 256 + threadIdx.x;      // position in s_k
-            const int64_t i = base + j * 256 + threadIdx.x;
-            if (i >= n) continue;
-            const uint32_t key = s_k[q], bu = key >> BKT_SHIFT;
-            int lo = q, hi = q + 1, seen = 1;
+#pragma unroll
+        for (int j = 0; j < PART_SUB_ITEMS; j++) {
+            const int q = j * 256 + threadIdx.x;
+            if (q < m) s_st[s_off[key[j] >> W] + rank[j]] = make_uint2(key[j], (uint32_t)(s0 + q));
+        }
+        __syncthreads();
+        for (int q = threadIdx.x; q < m; q += 256) {
+            const uint2 pr = s_st[q];
+            const uint32_t p = pr.x >> W;
+            pairs[s_cur[p] + (uint32_t)q - s_off[p]] = pr;
+        }
+        __syncthreads();
+        for (int p = threadIdx.x; p < P; p += 256) s_cur[p] += (p + 1 < PART_MAX ? s_off[p + 1] : (uint32_t)m) - s_off[p];
+        __syncthreads();
+    }
+}
+
+// One partition per CTA iteration (partitions taken by ticket, in order):
+//   1. 256-bp bucket histogram of the partition in shared memory, turned into an inclusive prefix (warp w owns the w-th
+//      eighth of the buckets; pre(i) adds the warp bases)
+//   2. flag of every bucket: the +-rb bucket window holds >= need signatures, the halo taken from the neighbours' edge
+//      counts -- the same rule as a genome-wide histogram; survivor total published to the look-back at once
+//   3. exclusive offsets of the flagged buckets, in place; the pairs are streamed again and every survivor is put into
+//      its bucket's slot range in the shared-memory stage (more than PF_STAGE survivors: in `spill`, at the output's offsets)
+//   4. order inside every bucket: rank against the bucket (<= FIX_SMALL members), or a CTA counting sort on the low
+//      BKT_SHIFT bits for larger buckets -> keys_out / idx_out at the partition's survivor base
+__global__ void __launch_bounds__(256) k_part_filter(const uint2* __restrict__ pairs, const uint32_t* __restrict__ base, int P, int W, int rb,
+                                                     uint32_t need, const uint32_t* __restrict__ edge, uint32_t* __restrict__ keys_out,
+                                                     uint32_t* __restrict__ idx_out, uint2* __restrict__ spill, uint32_t* n_out, TileSync ts) {
+    pdl_launch_dependents(); pdl_wait();
+    extern __shared__ __align__(16) uint32_t s_dyn[];
+    const int BP = 1 << (W - BKT_SHIFT), WSH = W - BKT_SHIFT - 3, BPW = 1 << WSH;   // BPW buckets per warp
+    uint32_t* s_h = s_dyn;                                        // BP words
+    uint32_t* s_f = s_dyn + BP;                                   // BP / 32 flag words
+    uint2* s_st = reinterpret_cast<uint2*>(s_dyn + BP + BP / 32); // PF_STAGE pairs
+    __shared__ uint32_t s_warp[9], s_wb[9], s_fb[9];
+    __shared__ uint32_t s_hl[BKT_PAD + 1], s_hr[BKT_PAD + 1];
+    __shared__ uint32_t s_big[PF_BIG_CAP], s_cnt[256];
+    __shared__ uint32_t s_tile, s_excl, s_nbig;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint32_t gen = ts_gen(ts);
+    const uint32_t bmask = BP - 1;
+    while (true) {
+        if (threadIdx.x == 0) { s_tile = atomicAdd(ts.ticket, 1u); s_nbig = 0; }
+        for (int i = threadIdx.x; i < BP; i += 256) s_h[i] = 0;
+        __syncthreads();
+        const int p = (int)s_tile;
+        if (p >= P) break;
+        if (warp < 2) {   // halo prefixes: s_hl[k] = the k last buckets of p-1, s_hr[k] = the k first buckets of p+1
+            const int q = warp == 0 ? p - 1 : p + 1;
+            const uint32_t* e = edge + (int64_t)q * 2 * BKT_PAD + (warp == 0 ? BKT_PAD : 0);
+            const bool ok = q >= 0 && q < P;
+            uint32_t v0 = ok && lane < rb ? e[lane] : 0u, v1 = ok && lane + 32 < rb ? e[lane + 32] : 0u;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const uint32_t y0 = __shfl_up_sync(0xffffffffu, v0, d), y1 = __shfl_up_sync(0xffffffffu, v1, d);
+                if (lane >= d) { v0 += y0; v1 += y1; }
+            }
+            v1 += __shfl_sync(0xffffffffu, v0, 31);
+            uint32_t* h = warp == 0 ? s_hl : s_hr;
+            h[lane + 1] = v0; h[lane + 33] = v1;
+            if (lane == 0) h[0] = 0;
+        }
+        const int64_t lo = base[p], cnt = (int64_t)base[p + 1] - lo;
+        const uint2* src_pairs = pairs + lo;
+        // 1. histogram
+        constexpr int U = 8;   // loads in flight per thread
+        for (int64_t i0 = threadIdx.x; i0 < cnt; i0 += 256 * U) {
+            uint32_t k[U];
+#pragma unroll
+            for (int u = 0; u < U; u++) k[u] = i0 + u * 256 < cnt ? src_pairs[i0 + u * 256].x : 0u;
+#pragma unroll
+            for (int u = 0; u < U; u++)
+                if (i0 + u * 256 < cnt) atomicAdd(&s_h[(k[u] >> BKT_SHIFT) & bmask], 1u);
+        }
+        __syncthreads();
+        {   // inclusive prefix inside every warp's range
+            uint32_t run = 0;
+            for (int b = warp * BPW + lane; b < (warp + 1) * BPW; b += 32) {
+                uint32_t v = s_h[b];
+#pragma unroll
+                for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, v, d); if (lane >= d) v += y; }
+                s_h[b] = run + v;
+                run += __shfl_sync(0xffffffffu, v, 31);
+            }
+            if (lane == 0) s_warp[warp] = run;
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            uint32_t r = 0;
+            for (int w = 0; w < 8; w++) { s_wb[w] = r; r += s_warp[w]; }
+            s_wb[8] = r;
+        }
+        __syncthreads();
+        auto pre = [&](int i) -> uint32_t { return i < 0 ? 0u : s_h[i] + s_wb[i >> WSH]; };   // buckets [0, i]
+        // 2. flags and the survivors of every warp's range
+        {
+            uint32_t mine = 0;
+            for (int b = warp * BPW + lane; b < (warp + 1) * BPW; b += 32) {
+                const uint32_t c = pre(b) - pre(b - 1);
+                uint32_t win = pre(min(b + rb, BP - 1)) - pre(b - rb - 1);
+                if (b < rb) win += s_hl[rb - b];
+                if (b + rb >= BP) win += s_hr[b + rb - BP + 1];
+                const bool f = c > 0 && win >= need;
+                const uint32_t bits = __ballot_sync(0xffffffffu, f);
+                if (lane == 0) s_f[b >> 5] = bits;
+                if (f) mine += c;
+            }
+#pragma unroll
+            for (int d = 16; d > 0; d >>= 1) mine += __shfl_xor_sync(0xffffffffu, mine, d);
+            if (lane == 0) s_warp[warp] = mine;
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            uint32_t r = 0;
+            for (int w = 0; w < 8; w++) { s_fb[w] = r; r += s_warp[w]; }
+            s_fb[8] = r;
+        }
+        __syncthreads();
+        const uint32_t S = s_fb[8];
+        if (warp == 0) {   // publish the partition's survivor count at once, then wait for the base
+            const uint32_t ex = lookback_exclusive_warp(ts.status, gen, p, S);
+            if (lane == 0) { s_excl = ex; if (S) atomicAdd(n_out, S); }
+        }
+        {   // 3a. exclusive offsets of the flagged buckets, in place (a warp reads and writes only its own range)
+            uint32_t run = s_fb[warp], prev = s_wb[warp];
+            for (int b = warp * BPW + lane; b < (warp + 1) * BPW; b += 32) {
+                const uint32_t pb = s_h[b] + s_wb[warp];
+                uint32_t pm = __shfl_up_sync(0xffffffffu, pb, 1);
+                if (lane == 0) pm = prev;
+                prev = __shfl_sync(0xffffffffu, pb, 31);
+                const uint32_t c = ((s_f[b >> 5] >> lane) & 1u) ? pb - pm : 0u;
+                uint32_t v = c;
+#pragma unroll
+                for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, v, d); if (lane >= d) v += y; }
+                s_h[b] = run + v - c;
+                run += __shfl_sync(0xffffffffu, v, 31);
+                if (c > FIX_SMALL) {
+                    const uint32_t q = atomicAdd(&s_nbig, 1u);
+                    if (q < PF_BIG_CAP) s_big[q] = b;
+                }
+            }
+        }
+        __syncthreads();
+        const uint32_t obase = s_excl;
+        const bool spilled = S > (uint32_t)PF_STAGE;
+        uint2* st = spilled ? spill + obase : s_st;
+        // 3b. survivors into their buckets' slot ranges (afterwards s_h[b] = end of bucket b)
+        for (int64_t i0 = threadIdx.x; i0 < cnt; i0 += 256 * U) {
+            uint2 pr[U];
+#pragma unroll
+            for (int u = 0; u < U; u++) pr[u] = i0 + u * 256 < cnt ? src_pairs[i0 + u * 256] : make_uint2(0u, 0u);
+#pragma unroll
+            for (int u = 0; u < U; u++) {
+                const uint32_t b = (pr[u].x >> BKT_SHIFT) & bmask;
+                if (i0 + u * 256 < cnt && ((s_f[b >> 5] >> (b & 31)) & 1u)) st[atomicAdd(&s_h[b], 1u)] = pr[u];
+            }
+        }
+        __syncthreads();
+        // 4a. small buckets: rank against the bucket, ties by slot
+        for (uint32_t q = threadIdx.x; q < S; q += 256) {
+            const uint2 pr = st[q];
+            const uint32_t b = (pr.x >> BKT_SHIFT) & bmask;
+            const uint32_t beg = b ? s_h[b - 1] : 0u, end = s_h[b];
+            if (end - beg > FIX_SMALL) continue;
             uint32_t rank = 0;
-            const int qmin = (int)(base - FIX_SMALL < 0 ? FIX_SMALL - base : 0);                       // first valid position
-            const int64_t last = n - (base - FIX_SMALL);                                               // one past the last valid position
-            const int qmax = (int)(last < FX_TILE + 2 * FIX_SMALL ? last : FX_TILE + 2 * FIX_SMALL);
-            while (lo > qmin && seen <= FIX_SMALL) {
-                const uint32_t k = s_k[lo - 1];
-                if ((k >> BKT_SHIFT) != bu) break;
-                rank += k <= key ? 1u : 0u;     // earlier slot: smaller (key, slot) iff key <= mine
-                lo--; seen++;
+            for (uint32_t j = beg; j < end; j++) {
+                const uint32_t k = st[j].x;
+                rank += (k < pr.x || (k == pr.x && j < q)) ? 1u : 0u;
             }
-            while (hi < qmax && seen <= FIX_SMALL) {
-                const uint32_t k = s_k[hi];
-                if ((k >> BKT_SHIFT) != bu) break;
-                rank += k < key ? 1u : 0u;
-                hi++; seen++;
-            }
-            if (seen > FIX_SMALL) continue;     // a big bucket: ordered by k_bucket_fixup_big
-            const int64_t dst = base - FIX_SMALL + lo + rank;
-            keys_out[dst] = key;
-            idx_out[dst] = pairs[i].y;
+            keys_out[obase + beg + rank] = pr.x;
+            idx_out[obase + beg + rank] = pr.y;
         }
-        __syncthreads();
-    }
-    // big buckets (pile-ups, listed by k_bucket_prefix): one CTA per bucket, counting sort on the low BKT_SHIFT bits
-    constexpr int NB = 1 << BKT_SHIFT;
-    static_assert(NB == 256, "one histogram bin per thread");
-    uint32_t* s_cnt = s_k;
-    const uint32_t n_list = min(*BB.count, BB.cap);
-    for (uint32_t q = blockIdx.x; q < n_list; q += gridDim.x) {
-        const uint4 e = BB.list[q];
-        const uint32_t first = tile_base[e.x] + e.y, cnt = e.z;
-        s_cnt[threadIdx.x] = 0;
-        __syncthreads();
-        for (uint32_t i = threadIdx.x; i < cnt; i += 256) atomicAdd(&s_cnt[pairs[first + i].x & (NB - 1)], 1u);
-        __syncthreads();
-        uint32_t total;
-        const uint32_t ex = block_excl_scan_256(s_cnt[threadIdx.x], s_warp, &total);
-        s_cnt[threadIdx.x] = ex;
-        __syncthreads();
-        for (uint32_t i = threadIdx.x; i < cnt; i += 256) {
-            const uint2 pr = pairs[first + i];
-            const uint32_t dst = first + atomicAdd(&s_cnt[pr.x & (NB - 1)], 1u);
-            keys_out[dst] = pr.x;
-            idx_out[dst] = pr.y;
+        // 4b. large buckets: counting sort on the low BKT_SHIFT bits, one bucket at a time
+        static_assert((1 << BKT_SHIFT) == 256, "one counting-sort bin per thread");
+        const uint32_t nbig = s_nbig;
+        const uint32_t nb = nbig <= (uint32_t)PF_BIG_CAP ? nbig : (uint32_t)BP;   // list overflow: visit every bucket
+        for (uint32_t k = 0; k < nb; k++) {
+            const uint32_t b = nbig <= (uint32_t)PF_BIG_CAP ? s_big[k] : k;
+            const uint32_t beg = b ? s_h[b - 1] : 0u, end = s_h[b];
+            if (end - beg <= FIX_SMALL) continue;   // (uniform across the CTA)
+            __syncthreads();
+            s_cnt[threadIdx.x] = 0;
+            __syncthreads();
+            for (uint32_t j = beg + threadIdx.x; j < end; j += 256) atomicAdd(&s_cnt[st[j].x & 255u], 1u);
+            __syncthreads();
+            uint32_t total;
+            const uint32_t ex = block_excl_scan_256(s_cnt[threadIdx.x], s_warp, &total);
+            s_cnt[threadIdx.x] = ex;
+            __syncthreads();
+            for (uint32_t j = beg + threadIdx.x; j < end; j += 256) {
+                const uint2 pr = st[j];
+                const uint32_t d = obase + beg + atomicAdd(&s_cnt[pr.x & 255u], 1u);
+                keys_out[d] = pr.x;
+                idx_out[d] = pr.y;
+            }
         }
         __syncthreads();
     }
 }
+
 // small types: three sort keys per signature (name, second coordinate, primary)
 __global__ void k_other_keys(const int32_t* __restrict__ chrom, const int32_t* __restrict__ a, const int32_t* __restrict__ b,
                              const int32_t* __restrict__ rid, const int32_t* __restrict__ c, int64_t n, int svtype, ContigTab ct,
