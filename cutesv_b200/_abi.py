@@ -71,7 +71,15 @@ GENO_DTYPE = np.dtype([
     ("dr", "<i4"), ("dv", "<i4"), ("gt", "<i4"), ("pl", "<i4", (3,)), ("gq", "<i4"),
     ("status", "<i4"), ("qual", "<f8"),
 ])
-assert CAND_DTYPE.itemsize == 64 and GENO_DTYPE.itemsize == 40
+WINDOW_DTYPE = np.dtype([("chrom", "<i4"), ("reserved", "<i4"), ("s2", "<i8"), ("e2", "<i8")])   # csv_window, half units
+assert CAND_DTYPE.itemsize == 64 and GENO_DTYPE.itemsize == 40 and WINDOW_DTYPE.itemsize == 24
+
+
+def make_windows(chrom, s2, e2):
+    """csv_window array from contig ids and half-unit bounds."""
+    w = np.zeros(len(s2), dtype=WINDOW_DTYPE)
+    w["chrom"], w["s2"], w["e2"] = chrom, s2, e2
+    return w
 
 
 def i32(a):

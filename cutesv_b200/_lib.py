@@ -41,6 +41,9 @@ _SIGNATURES = {
     "csv_cluster_host_grouped": (C.c_int, [_VP, C.POINTER(_abi.csv_sig_cols), C.POINTER(_I64P), C.POINTER(_abi.csv_reads_cols), _I64P,
                                            C.c_uint32, _VP, _VP, C.c_int64, _I32P, C.c_int64, _I64P, _I64P]),
     "csv_cal_gl": (C.c_int, [_VP, _I32P, _I32P, C.c_int64, _VP]),
+    "csv_overlap_cover": (C.c_int, [_VP, _VP, C.c_int64, C.POINTER(_abi.csv_reads_cols), _I32P, _I32P, _I64P, _I32P, C.c_int64, _I64P, _I32P,
+                                    C.c_int64, _I64P, _I64P]),
+    "csv_call_gt": (C.c_int, [_VP, _VP, C.c_int64, C.c_int32, C.POINTER(_abi.csv_reads_cols), _I64P, _I32P, _VP]),
     "csv_extract": (C.c_int, [_VP, C.POINTER(_abi.csv_read_cols), C.POINTER(C.c_uint32), C.c_int64,
                               C.POINTER(_abi.csv_sa_cols), _I64P, _I64P]),
     "csv_extract_append": (C.c_int, [_VP, C.POINTER(_abi.csv_read_cols), C.POINTER(C.c_uint32), C.c_int64,

@@ -1165,4 +1165,59 @@ CSV_HD void tra_call_gt(const AlnView& A, const csv_cand& c, const int32_t* sup,
     g->dr = dr; g->dv = n_sup;
 }
 
+// ------------------------------------------------------------------------------------------
+// standalone overlap_cover (cuteSV_genotype.py:95-159) over arbitrary windows and reads rows, in half units
+// (window (s2, e2) = 2 * (s, e), read (2 * start, 2 * end)).  The event order sv-right 0 < read-left 1 <
+// read-right 2 < sv-left 3 makes a row overlap a window iff start < e and end > s, and cover it iff
+// start <= s and end >= e (end > s follows from e > s, which the caller guarantees).
+// ------------------------------------------------------------------------------------------
+CSV_HD bool gc_overlaps(int64_t rs2, int64_t re2, int64_t s2, int64_t e2) { return rs2 < e2 && re2 > s2; }
+CSV_HD bool gc_covers(int64_t rs2, int64_t re2, int64_t s2, int64_t e2) { return rs2 <= s2 && re2 >= e2 && re2 > s2; }
+// Bins of 2^GC_SHIFT half units per contig; coordinates below 0 fall into bin 0.  A window is listed in every bin of
+// [s2, e2 - 1], a row visits every bin of [rs2, re2].  An overlapping pair is taken in one bin only, that of
+// max(rs2, s2): the point lies in both ranges, so both sides reach that bin.
+static constexpr int GC_SHIFT = 12;
+CSV_HD int64_t gc_bin(int64_t x2) { return x2 < 0 ? 0 : (x2 >> GC_SHIFT); }
+CSV_HD bool gc_pair_home(int64_t rs2, int64_t s2, int64_t bin) { return gc_bin(rs2 > s2 ? rs2 : s2) == bin; }
+
+// Sort + deduplicate one segment of name ids (a window's cover or overlap list) into out[0, k), ascending; returns k.
+// Team-parallel rank sort: first[i] marks the first occurrence of a value, and a first occurrence goes to the number of
+// distinct smaller values.  O(n^2 / team size): a warp takes short segments, a CTA the pile-ups.  `first` holds n bytes.
+template <class Team>
+CSV_HD int gc_sort_unique(const Team& tm, const int32_t* in, int n, uint8_t* first, int32_t* out) {
+    for (int i = tm.tid(); i < n; i += Team::SIZE) {
+        const int32_t v = in[i];
+        bool f = true;
+        for (int j = 0; j < i && f; j++) f = in[j] != v;
+        first[i] = f ? 1 : 0;
+    }
+    tm.sync();
+    for (int i = tm.tid(); i < n; i += Team::SIZE) {
+        if (!first[i]) continue;
+        const int32_t v = in[i];
+        int pos = 0;
+        for (int j = 0; j < n; j++) pos += (first[j] && in[j] < v) ? 1 : 0;
+        out[pos] = v;
+    }
+    int k = 0;
+    for (int j = 0; j < n; j++) k += first[j];
+    tm.sync();
+    return k;
+}
+
+// assign_gt's DR for one candidate (cuteSV_genotype.py:161-173, windows united as in resolveDUP.py:155-157):
+// |a ∪ b \ sup| for ascending unique a, b and ascending sup (duplicates allowed).
+CSV_HD int32_t gc_union_minus(const int32_t* a, int na, const int32_t* b, int nb, const int32_t* sup, int nsup) {
+    int32_t dr = 0;
+    int i = 0, j = 0;
+    while (i < na || j < nb) {
+        int32_t v;
+        if (j >= nb || (i < na && a[i] < b[j])) v = a[i++];
+        else if (i >= na || b[j] < a[i]) v = b[j++];
+        else { v = a[i++]; j++; }
+        if (!sorted_contains(sup, nsup, v)) dr++;
+    }
+    return dr;
+}
+
 }  // namespace csv

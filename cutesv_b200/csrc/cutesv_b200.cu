@@ -117,6 +117,19 @@ struct LaneWork {
     DBuf boff, rec_a, rec_b, recc_a, recc_b, rest_list;   // partitioned INS/DEL front end, k_cluster_small's rest list
     SmallWork small;
 };
+// scratch of csv_overlap_cover / csv_call_gt (genotype_api.inl): separate from everything csv_cluster uses
+struct GcWork {
+    DBuf win, bin_base, bin_start, bin_fill, bin_list, iter, prim, cov_off, ovl_off, cov_fill, ovl_fill, cov_u, ovl_u, lb, words;
+    DBuf r_chrom, r_start, r_end, r_id, r_prim, cov_raw, ovl_raw, cov_ded, ovl_ded, cov_flag, ovl_flag, sup_off, sup, geno;
+    uint32_t n_cov = 0, n_ovl = 0;   // raw ids of the last call
+    void release() {
+        DBuf* all[] = {&win, &bin_base, &bin_start, &bin_fill, &bin_list, &iter, &prim, &cov_off, &ovl_off, &cov_fill, &ovl_fill, &cov_u, &ovl_u,
+                       &lb, &words, &r_chrom, &r_start, &r_end, &r_id, &r_prim, &cov_raw, &ovl_raw, &cov_ded, &ovl_ded, &cov_flag, &ovl_flag,
+                       &sup_off, &sup, &geno};
+        for (DBuf* b : all) b->release();
+    }
+};
+
 static constexpr int N_LANES = CSV_NTYPES;
 static inline int lane_of(int t) { return t; }
 
@@ -233,6 +246,7 @@ struct csv_ctx {
                                         // other lanes' kernels need
     bool prev_is_chain_kernel = false;  // the launch being enqueued directly follows a chain kernel on the same stream
     DBuf cal_in0, cal_in1, cal_out, aln_flag;   // csv_cal_gl / csv_upload_alignments scratch (no per-call cudaMalloc)
+    GcWork gc;                                  // csv_overlap_cover / csv_call_gt
     int64_t pad_cand = 0, pad_names = 0;
     int64_t* h_gather = nullptr;    // pinned: per-rank headers after the gather
     int64_t g_n_cand = 0, g_n_names = 0;
@@ -481,6 +495,7 @@ extern "C" int csv_destroy(csv_ctx* c) {
                    &c->d_len_eff, &c->g_send, &c->g_recv, &c->g_cand, &c->g_geno, &c->g_names, &c->g_scratch, &c->g_tab, &c->cal_in0, &c->cal_in1,
                    &c->cal_out, &c->aln_flag, &c->scan_carry, &c->win_rec, &c->rest_list, &c->emit_cursor};
     for (DBuf* b : all) b->release();
+    c->gc.release();
     for (auto& g : c->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
     if (c->comm) comm_destroy(c);
     if (c->h_gather) cudaFreeHost(c->h_gather);
@@ -1566,3 +1581,4 @@ extern "C" int csv_sort_probe(csv_ctx* c, float* ms_total, int64_t* bytes_total,
 
 #include "extract_api.inl"
 #include "gather_api.inl"
+#include "genotype_api.inl"

@@ -1449,4 +1449,121 @@ __global__ void k_cal_gl(const int32_t* c0, const int32_t* c1, int64_t n, const 
     }
 }
 
+// ---- standalone overlap_cover / call_gt (csv_overlap_cover, csv_call_gt) ----
+// Windows are listed in every bin they span (per-contig bin ranges from bin_base), so a row that starts inside a window
+// finds it too; every (row, window) pair is taken once, in the bin of max(row start, window start) (core.h gc_*).
+// A count pass, exclusive scans and a fill pass build per-window CSR lists of name ids; each segment is then sorted and
+// deduplicated by one warp (short) or one CTA (pile-ups).
+struct GcJob {
+    const csv_window* win;
+    uint32_t n_win;
+    const uint32_t* bin_base;   // n_wc + 1: first bin of every window contig
+    int32_t n_wc;
+    uint32_t* bin_start;        // counts, then exclusive offsets (n_bins + 1)
+    uint32_t* bin_fill;
+    uint32_t* bin_list;         // window ids grouped by bin
+    uint32_t* iter;             // overlapping rows per window
+    uint32_t* prim;             // overlapping primary rows per window
+    uint32_t* cov_off;          // counts, then raw segment offsets (n_win + 1)
+    uint32_t* ovl_off;
+    uint32_t* cov_fill;
+    uint32_t* ovl_fill;
+    int32_t* cov_raw;           // name ids, unordered inside a segment
+    int32_t* ovl_raw;
+    int want_overlap;
+};
+struct GcReads { const int32_t *chrom, *start, *end, *rid; const uint8_t* prim; int64_t n; };
+
+template <int PASS>
+__global__ void __launch_bounds__(256) k_gc_win_bins(GcJob J) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < J.n_win; i += gridDim.x * blockDim.x) {
+        const csv_window w = J.win[i];
+        const uint32_t base = J.bin_base[w.chrom];
+        const uint32_t b0 = base + (uint32_t)gc_bin(w.s2), b1 = base + (uint32_t)gc_bin(w.e2 - 1);
+        for (uint32_t b = b0; b <= b1; b++) {
+            if (PASS == 0) atomicAdd(&J.bin_start[b], 1u);
+            else J.bin_list[J.bin_start[b] + atomicAdd(&J.bin_fill[b], 1u)] = i;
+        }
+    }
+}
+
+// one thread per row: PASS 0 counts, PASS 1 writes the name ids of primary rows into the raw segments
+template <int PASS>
+__global__ void __launch_bounds__(256) k_gc_pairs(GcJob J, GcReads R, uint32_t* status) {
+    for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < R.n; r += (int64_t)gridDim.x * blockDim.x) {
+        const int32_t ch = R.chrom[r], st = R.start[r], en = R.end[r];
+        if (ch < 0 || en < st) { if (PASS == 0) atomicOr(status, ch < 0 ? ST_BAD_CHROM : ST_BAD_POS); continue; }
+        if (ch >= J.n_wc) continue;
+        const uint32_t base = J.bin_base[ch], nb = J.bin_base[ch + 1] - base;
+        const int64_t rs2 = 2 * (int64_t)st, re2 = 2 * (int64_t)en;
+        const int64_t b0 = gc_bin(rs2);
+        if ((uint64_t)b0 >= nb) continue;
+        int64_t b1 = gc_bin(re2);
+        if (b1 >= (int64_t)nb) b1 = nb - 1;
+        const bool pr = R.prim[r] != 0;
+        const int32_t rid = R.rid[r];
+        for (int64_t b = b0; b <= b1; b++) {
+            const uint32_t k1 = J.bin_start[base + b + 1];
+            for (uint32_t k = J.bin_start[base + b]; k < k1; k++) {
+                const uint32_t wi = J.bin_list[k];
+                const csv_window w = J.win[wi];
+                if (!gc_overlaps(rs2, re2, w.s2, w.e2) || !gc_pair_home(rs2, w.s2, b)) continue;
+                const bool cov = pr && gc_covers(rs2, re2, w.s2, w.e2);
+                if (PASS == 0) {
+                    atomicAdd(&J.iter[wi], 1u);
+                    if (pr) atomicAdd(&J.prim[wi], 1u);
+                    if (pr && J.want_overlap) atomicAdd(&J.ovl_off[wi], 1u);
+                    if (cov) atomicAdd(&J.cov_off[wi], 1u);
+                } else {
+                    if (pr && J.want_overlap) J.ovl_raw[J.ovl_off[wi] + atomicAdd(&J.ovl_fill[wi], 1u)] = rid;
+                    if (cov) J.cov_raw[J.cov_off[wi] + atomicAdd(&J.cov_fill[wi], 1u)] = rid;
+                }
+            }
+        }
+    }
+}
+
+// Sort + deduplicate segments [off[k], off[k+1]) of raw into ded at the same offsets; ucnt[k] = distinct ids.
+// k_gc_dedup_warp takes the segments of at most GC_WARP_SEG ids, k_gc_dedup_cta the longer ones.
+static constexpr uint32_t GC_WARP_SEG = 64;
+__global__ void __launch_bounds__(256) k_gc_dedup_warp(const uint32_t* __restrict__ off, const int32_t* raw, uint32_t n_seg, uint8_t* flag,
+                                                       int32_t* ded, uint32_t* ucnt) {
+    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, n_warps = (gridDim.x * blockDim.x) >> 5;
+    CudaTeam<32> tm;
+    for (uint32_t k = warp; k < n_seg; k += n_warps) {
+        const uint32_t o = off[k], n = off[k + 1] - o;
+        if (n > GC_WARP_SEG) continue;
+        const int u = gc_sort_unique(tm, raw + o, (int)n, flag + o, ded + o);
+        if (tm.tid() == 0) ucnt[k] = (uint32_t)u;
+    }
+}
+__global__ void __launch_bounds__(256) k_gc_dedup_cta(const uint32_t* __restrict__ off, const int32_t* raw, uint32_t n_seg, uint8_t* flag,
+                                                      int32_t* ded, uint32_t* ucnt) {
+    CudaTeam<256> tm;
+    for (uint32_t k = blockIdx.x; k < n_seg; k += gridDim.x) {
+        const uint32_t o = off[k], n = off[k + 1] - o;
+        if (n <= GC_WARP_SEG) continue;
+        const int u = gc_sort_unique(tm, raw + o, (int)n, flag + o, ded + o);
+        if (tm.tid() == 0) ucnt[k] = (uint32_t)u;
+    }
+}
+
+// call_gt's genotype per candidate: DR from the deduplicated cover segments of its windows (per consecutive windows,
+// united) minus its ascending support ids, DV = support list length, then cal_GL from the table
+__global__ void __launch_bounds__(256) k_gc_call_gt(const uint32_t* __restrict__ cov_off, const uint32_t* __restrict__ cov_u,
+                                                    const int32_t* __restrict__ ded, int64_t n_cand, int per,
+                                                    const int64_t* __restrict__ sup_off, const int32_t* __restrict__ sup,
+                                                    const csv_geno* __restrict__ gl_table, csv_geno* __restrict__ out) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_cand; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t w0 = i * per, w1 = per == 2 ? w0 + 1 : w0;
+        const int n1 = per == 2 ? (int)cov_u[w1] : 0;
+        const int64_t so = sup_off[i];
+        const int32_t dv = (int32_t)(sup_off[i + 1] - so);
+        const int32_t dr = gc_union_minus(ded + cov_off[w0], (int)cov_u[w0], ded + cov_off[w1], n1, sup + so, dv);
+        csv_geno g = gl_table[gl_index(dr, dv)];
+        g.dr = dr; g.dv = dv;
+        out[i] = g;
+    }
+}
+
 }  // namespace csv

@@ -1,7 +1,8 @@
-"""Drop-in for the reference's cuteSV_resolveINDEL (resolveINDEL.py:17-108, 222-317, 435-439):
+"""Drop-in for the reference's cuteSV_resolveINDEL (resolveINDEL.py:17-108, 222-317, 435-479):
 same names, same argument meaning, same returned rows -- computed by the CUDA path."""
-from . import _abi
+from . import _abi, workdir
 from ._resolve_common import resolve_one
+from .cuteSV_genotype import call_gt_genos, geno_fields
 
 
 def resolution_DEL(path, chr, svtype, read_count, threshold_gloab, max_cluster_bias, minimum_support_reads, bam_path, action,
@@ -26,3 +27,20 @@ def run_del(args):
 
 def run_ins(args):
     return resolution_INS(*args)
+
+
+def call_gt(temporary_dir, chr, candidate_single_SV, max_cluster_bias, svtype, sigs_index):
+    """Genotyped rows of resolveINDEL.py:441-479: candidates [chr, svtype, pos, len, support, CIPOS, CILEN, search position,
+    read names(, INS sequence)], DR counted over the window search position +- max_cluster_bias."""
+    if chr not in sigs_index["reads"].keys():
+        return []
+    reads_list = workdir.load_slice(temporary_dir, "reads", chr, sigs_index)
+    svs_list = [(max(item[7] - max_cluster_bias, 0), item[7] + max_cluster_bias) for item in candidate_single_SV]
+    genos = call_gt_genos(reads_list, svs_list, 1, [item[8] for item in candidate_single_SV])
+    out = []
+    for item, g in zip(candidate_single_SV, genos):
+        row = [item[0], item[1], str(item[2]), str(item[3]), str(item[4]), item[5], item[6]] + list(geno_fields(g)) + [",".join(item[8])]
+        if svtype == "INS":
+            row.append(item[9])
+        out.append(row)
+    return out

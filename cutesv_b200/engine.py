@@ -155,6 +155,54 @@ class Engine(object):
         _lib.check(self.L.csv_cal_gl(self.h, _abi.ptr(c0), _abi.ptr(c1), C.c_int64(len(c0)), out.ctypes.data_as(C.c_void_p)))
         return out
 
+    def overlap_cover(self, windows, reads=None, overlap=True):
+        """overlap_cover (cuteSV_genotype.py:95-159) on the device.  windows: _abi.WINDOW_DTYPE array (half units); reads: dict
+        (chrom, start, end, read_id, is_primary) or None for the device-resident reads table.  Returns dict(iteration, primary_num,
+        cover_off, cover_ids[, overlap_off, overlap_ids]): per window the overlapping rows, the overlapping primary rows and the
+        ascending distinct read ids of the primary covering / overlapping rows as CSR."""
+        w = np.ascontiguousarray(windows, dtype=_abi.WINDOW_DTYPE)
+        n = len(w)
+        r, keep = _abi.make_reads_cols(reads) if reads is not None else (None, ())
+        it = np.zeros(max(n, 1), np.int32)
+        pn = np.zeros(max(n, 1), np.int32)
+        co = np.zeros(n + 1, np.int64)
+        oo = np.zeros(n + 1, np.int64)
+        cap_c = cap_o = 4 * n + 1024
+        nc, no = C.c_int64(0), C.c_int64(0)
+        while True:
+            ci = np.zeros(cap_c, np.int32)
+            oi = np.zeros(cap_o, np.int32) if overlap else None
+            rc = self.L.csv_overlap_cover(self.h, w.ctypes.data_as(C.c_void_p), C.c_int64(n), C.byref(r) if r is not None else None, _abi.ptr(it),
+                                          _abi.ptr(pn), co.ctypes.data_as(C.POINTER(C.c_int64)), _abi.ptr(ci), C.c_int64(cap_c),
+                                          oo.ctypes.data_as(C.POINTER(C.c_int64)), _abi.ptr(oi), C.c_int64(cap_o if overlap else 0),
+                                          C.byref(nc), C.byref(no))
+            if rc != _abi.CSV_E_CAPACITY:
+                break
+            cap_c, cap_o = max(cap_c, nc.value), max(cap_o, no.value)
+        _lib.check(rc)
+        del keep
+        out = dict(iteration=it[:n], primary_num=pn[:n], cover_off=co, cover_ids=ci[:nc.value])
+        if overlap:
+            out.update(overlap_off=oo, overlap_ids=oi[:no.value])
+        return out
+
+    def call_gt(self, windows, windows_per_cand, support_off, support_ids, reads=None):
+        """call_gt + assign_gt (resolveINDEL.py:441, resolveDUP.py:137, resolveINV.py:208) on the device: candidate i owns windows
+        [i*windows_per_cand, (i+1)*windows_per_cand) (united cover sets) and support ids [support_off[i], support_off[i+1]).
+        Returns a GENO_DTYPE array: cal_GL(DR, DV) with dr / dv."""
+        w = np.ascontiguousarray(windows, dtype=_abi.WINDOW_DTYPE)
+        so = np.ascontiguousarray(support_off, dtype=np.int64)
+        si = np.ascontiguousarray(support_ids, dtype=np.int32)
+        n = len(so) - 1
+        assert len(w) == n * windows_per_cand
+        r, keep = _abi.make_reads_cols(reads) if reads is not None else (None, ())
+        out = np.zeros(max(n, 1), dtype=_abi.GENO_DTYPE)
+        _lib.check(self.L.csv_call_gt(self.h, w.ctypes.data_as(C.c_void_p), C.c_int64(n), C.c_int32(windows_per_cand),
+                                      C.byref(r) if r is not None else None, so.ctypes.data_as(C.POINTER(C.c_int64)), _abi.ptr(si),
+                                      out.ctypes.data_as(C.c_void_p)))
+        del keep
+        return out[:n]
+
     def stage_ms(self):
         ms = (C.c_float * _abi.CSV_ST_COUNT)()
         _lib.check(self.L.csv_stage_ms(self.h, ms))

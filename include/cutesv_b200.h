@@ -223,6 +223,39 @@ int csv_cluster_host_grouped(csv_ctx* ctx, const csv_sig_cols sigs[CSV_NTYPES], 
 /* cal_GL(c0=DR, c1=DV) (cuteSV_genotype.py:33-56) for n pairs, evaluated on the device. */
 int csv_cal_gl(csv_ctx* ctx, const int32_t* c0, const int32_t* c1, int64_t n, csv_geno* out);
 
+/* ---- standalone genotype helpers: overlap_cover (cuteSV_genotype.py:95-159) and the call_gt of resolveINDEL.py:441,
+ * resolveDUP.py:137 and resolveINV.py:208 over any window list and reads table (both may span several contigs) ----
+ *
+ * Coordinates are in half units, so that the x.5 windows of DUP / INV (bias/2) are exact: window [s, e] is
+ * (s2, e2) = (2s, 2e), a reads-table row [start, end] is compared as (2 start, 2 end).  A row overlaps a window iff
+ * start < e and end > s; it covers it iff start <= s and end >= e.  Only rows on the window's contig count.
+ *
+ * reads == NULL: the device-resident reads table of csv_extract* / csv_upload_reads*.  Neither call changes that table
+ * nor anything csv_cluster / csv_fetch return; both block until their results are on the host.
+ * Input errors (CSV_E_INPUT): a window with chrom < 0 or e2 <= s2 (the reference raises KeyError there), a reads row with
+ * chrom < 0 or end < start. */
+typedef struct csv_window {
+    int32_t chrom;    /* contig id, the same numbering as the reads table's chrom column */
+    int32_t reserved;
+    int64_t s2;       /* 2 * window start */
+    int64_t e2;       /* 2 * window end, > s2 */
+} csv_window;
+
+/* overlap_cover: iteration[i] = overlapping rows, primary_num[i] = overlapping rows with is_primary != 0;
+ * cover / overlap: per window the distinct read ids of the primary covering / overlapping rows, ascending, as CSR
+ * (cover_off / overlap_off: n_windows + 1 entries).  On CSV_E_CAPACITY *n_cover / *n_overlap hold the sizes needed.
+ * overlap_ids may be NULL (with cap_overlap 0) to skip the overlap lists; overlap_off is then left alone. */
+int csv_overlap_cover(csv_ctx* ctx, const csv_window* windows, int64_t n_windows, const csv_reads_cols* reads,
+                      int32_t* iteration, int32_t* primary_num, int64_t* cover_off, int32_t* cover_ids, int64_t cap_cover,
+                      int64_t* overlap_off, int32_t* overlap_ids, int64_t cap_overlap, int64_t* n_cover, int64_t* n_overlap);
+
+/* call_gt + assign_gt: n_cand candidates of windows_per_cand (1: DEL / INS, 2: DUP / INV breakpoints, whose cover
+ * sets are united) consecutive windows each; support_off (n_cand + 1) / support_ids: every candidate's supporting
+ * read ids in any order, duplicates allowed.  DR = |cover \ support|, DV = the support list's length,
+ * out[i] = cal_GL(DR, DV) with dr / dv filled. */
+int csv_call_gt(csv_ctx* ctx, const csv_window* windows, int64_t n_cand, int32_t windows_per_cand, const csv_reads_cols* reads,
+                const int64_t* support_off, const int32_t* support_ids, csv_geno* out);
+
 /* ---- signature extraction: parse_read / generate_combine_sigs / organize_split_signal /
  * analysis_split_read (cuteSV:50-681) over a packet of decoded alignment records ---- */
 
