@@ -478,6 +478,7 @@ extern "C" int csv_create(int device, void* stream, csv_ctx** out) {
     CU(cudaFuncSetAttribute(k_cluster_block<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, BLOCK_M * ARENA_PER_MAX));
     CU(cudaFuncSetAttribute(k_cluster_block<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, BLOCK_M * ARENA_PER_MAX));
     CU(cudaFuncSetAttribute(k_part_filter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pf_smem_bytes(PART_W_MAX)));
+    CU(cudaFuncSetAttribute(k_part_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ps_smem_bytes()));
     *out = c;
     return CSV_OK;
 }
@@ -963,11 +964,13 @@ static int run_indel(csv_ctx* c, int t, uint32_t kslot_base) {
         uint32_t* done_ctr = c->tickets.as<uint32_t>() + c->ticket_next++;
         CU(cudaMemsetAsync(edge, 0, edge_words * 4, c->stream));
         const int is_ins = t == CSV_INS ? 1 : 0;
+        if ((((uintptr_t)s.chrom.p) | ((uintptr_t)s.a.p)) & 15)   // k_part_scatter loads both columns 16 B at a time
+            return set_err(CSV_E_STATE, "signature columns are not 16 B aligned");
         LAUNCH(c, k_part_count, n_chunks, 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), n, is_ins, ct, W, P, n_chunks, rb, cnt, edge,
                &ctr->status);
         LAUNCH_PDL(c, k_part_scan, P, 256, 0, cnt, n_chunks, P, pbase, done_ctr);
         uint2* pairs = (uint2*)c->keys_a.p;   // 8 B per signature (ensure_lane_scratch)
-        LAUNCH_PDL(c, k_part_scatter, n_chunks, 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), n, is_ins, ct, W, P, n_chunks,
+        LAUNCH_PDL(c, k_part_scatter, n_chunks, 256, ps_smem_bytes(), s.chrom.as<int32_t>(), s.a.as<int32_t>(), n, is_ins, ct, W, P, n_chunks,
                    (const uint32_t*)cnt, (const uint32_t*)pbase, pairs);
         stage_end(c, CSV_ST_KEYS);
         stage_begin(c, CSV_ST_SORT);

@@ -397,46 +397,73 @@ __global__ void __launch_bounds__(256) k_part_scan(uint32_t* __restrict__ cnt, i
 }
 
 // (key, row) pairs grouped by partition; the order inside a partition is irrelevant (k_part_filter orders it).  The rows
-// of a chunk are grouped by partition in shared memory, PART_SUB at a time, so that every partition's run is written with
-// coalesced stores: single 8 B stores scattered over a buffer larger than L2 end up as partial-sector writes to DRAM.
-static constexpr int PART_SUB = 4096, PART_SUB_ITEMS = PART_SUB / 256;
-static_assert(PART_CHUNK % PART_SUB == 0 && PART_MAX == 4 * 256, "k_part_scatter tiling");
-__global__ void __launch_bounds__(256, 2) k_part_scatter(const int32_t* __restrict__ chrom, const int32_t* __restrict__ a, int64_t n, int is_ins,
+// of a chunk are grouped by partition in shared memory, PART_ROUND at a time, so that every partition's run is written with
+// coalesced stores: single 8 B stores scattered over a buffer larger than L2 end up as partial-sector writes to DRAM.  A
+// round of 8192 rows gives runs of about 11 pairs on permuted whole-genome input (P = 740); the stores of shorter runs
+// cost more than the loads.  A round issues all of its loads (16 B per column and thread, 8 of each) before the first key
+// is formed: the loads are the latency the kernel waits on, one round trip per round.  `chrom` and `a` must be 16 B
+// aligned (run_indel checks it); only the last 4-row group of the input is loaded row by row.
+static constexpr int PART_ROUND = 8192, PART_ROUND_V = PART_ROUND / 4 / 256;   // 4-row groups per thread and round
+static_assert(PART_CHUNK % PART_ROUND == 0 && PART_MAX == 4 * 256, "k_part_scatter tiling");
+__host__ __device__ constexpr size_t ps_smem_bytes() { return (size_t)PART_ROUND * 8 + (size_t)3 * PART_MAX * 4; }
+__global__ void __launch_bounds__(256) k_part_scatter(const int32_t* __restrict__ chrom, const int32_t* __restrict__ a, int64_t n, int is_ins,
                                                       ContigTab ct, int W, int P, int n_chunks, const uint32_t* __restrict__ cnt,
                                                       const uint32_t* __restrict__ base, uint2* __restrict__ pairs) {
     pdl_launch_dependents(); pdl_wait();
-    __shared__ uint32_t s_cur[PART_MAX];   // next slot of every partition in `pairs`
-    __shared__ uint32_t s_off[PART_MAX];   // rows of the sub-tile per partition -> their first position in s_st
-    __shared__ uint2 s_st[PART_SUB];
+    extern __shared__ __align__(16) uint32_t s_dyn[];
+    uint2* s_st = reinterpret_cast<uint2*>(s_dyn);   // PART_ROUND pairs, grouped by partition
+    uint32_t* s_cur = s_dyn + 2 * PART_ROUND;        // next slot of every partition in `pairs`
+    uint32_t* s_off = s_cur + PART_MAX;              // rows of the round per partition -> their first position in s_st
+    uint32_t* s_fill = s_off + PART_MAX;             // next free position of every partition in s_st
     __shared__ uint32_t s_warp[9];
     for (int p = threadIdx.x; p < P; p += blockDim.x) s_cur[p] = base[p] + cnt[(int64_t)p * n_chunks + blockIdx.x];
     const int64_t c1 = min((int64_t)(blockIdx.x + 1) * PART_CHUNK, n);
     uint32_t dummy = 0;   // validated by k_part_count
-    for (int64_t s0 = (int64_t)blockIdx.x * PART_CHUNK; s0 < c1; s0 += PART_SUB) {
-        const int m = (int)min((int64_t)PART_SUB, c1 - s0);
+    for (int64_t s0 = (int64_t)blockIdx.x * PART_CHUNK; s0 < c1; s0 += PART_ROUND) {   // s0 is a multiple of 4
+        const int m = (int)min((int64_t)PART_ROUND, c1 - s0);
+        // No barrier between the last round's s_cur update and this clear: both loops give partition p to thread p % 256
+        // (the kernel runs with 256 threads), so a thread clears only the s_off words it has just read.
         for (int p = threadIdx.x; p < PART_MAX; p += 256) s_off[p] = 0;
-        __syncthreads();
-        uint32_t key[PART_SUB_ITEMS], rank[PART_SUB_ITEMS];
+        int4 cv[PART_ROUND_V], av[PART_ROUND_V];   // rows s0 + r .. s0 + r + 3, r = 4 * (j * 256 + thread)
 #pragma unroll
-        for (int j = 0; j < PART_SUB_ITEMS; j++) {
-            const int q = j * 256 + threadIdx.x;
-            key[j] = q < m ? indel_key32(chrom[s0 + q], a[s0 + q], is_ins, ct, dummy) : 0u;
+        for (int j = 0; j < PART_ROUND_V; j++) {
+            const int r = 4 * (j * 256 + (int)threadIdx.x);
+            if (r + 4 <= m) {
+                cv[j] = __ldcs(reinterpret_cast<const int4*>(chrom + s0 + r));
+                av[j] = __ldcs(reinterpret_cast<const int4*>(a + s0 + r));
+            } else {
+                cv[j] = make_int4(r < m ? chrom[s0 + r] : 0, r + 1 < m ? chrom[s0 + r + 1] : 0, r + 2 < m ? chrom[s0 + r + 2] : 0,
+                                  r + 3 < m ? chrom[s0 + r + 3] : 0);
+                av[j] = make_int4(r < m ? a[s0 + r] : 0, r + 1 < m ? a[s0 + r + 1] : 0, r + 2 < m ? a[s0 + r + 2] : 0,
+                                  r + 3 < m ? a[s0 + r + 3] : 0);
+            }
         }
+        uint32_t key[4 * PART_ROUND_V];
 #pragma unroll
-        for (int j = 0; j < PART_SUB_ITEMS; j++)
-            if (j * 256 + (int)threadIdx.x < m) rank[j] = atomicAdd(&s_off[key[j] >> W], 1u);
+        for (int j = 0; j < PART_ROUND_V; j++) {
+            key[4 * j] = indel_key32(cv[j].x, av[j].x, is_ins, ct, dummy);
+            key[4 * j + 1] = indel_key32(cv[j].y, av[j].y, is_ins, ct, dummy);
+            key[4 * j + 2] = indel_key32(cv[j].z, av[j].z, is_ins, ct, dummy);
+            key[4 * j + 3] = indel_key32(cv[j].w, av[j].w, is_ins, ct, dummy);
+        }
+        __syncthreads();   // s_off cleared; the previous round's stores have read s_st
+#pragma unroll
+        for (int k = 0; k < 4 * PART_ROUND_V; k++)
+            if (4 * ((k >> 2) * 256 + (int)threadIdx.x) + (k & 3) < m) atomicAdd(&s_off[key[k] >> W], 1u);
         __syncthreads();
         {   // exclusive scan of the per-partition counts, four partitions per thread
             const uint4 v = reinterpret_cast<const uint4*>(s_off)[threadIdx.x];
             uint32_t total;
             const uint32_t ex = block_excl_scan_256(v.x + v.y + v.z + v.w, s_warp, &total);
-            reinterpret_cast<uint4*>(s_off)[threadIdx.x] = make_uint4(ex, ex + v.x, ex + v.x + v.y, ex + v.x + v.y + v.z);
+            const uint4 o = make_uint4(ex, ex + v.x, ex + v.x + v.y, ex + v.x + v.y + v.z);
+            reinterpret_cast<uint4*>(s_off)[threadIdx.x] = o;
+            reinterpret_cast<uint4*>(s_fill)[threadIdx.x] = o;
         }
         __syncthreads();
 #pragma unroll
-        for (int j = 0; j < PART_SUB_ITEMS; j++) {
-            const int q = j * 256 + threadIdx.x;
-            if (q < m) s_st[s_off[key[j] >> W] + rank[j]] = make_uint2(key[j], (uint32_t)(s0 + q));
+        for (int k = 0; k < 4 * PART_ROUND_V; k++) {
+            const int q = 4 * ((k >> 2) * 256 + (int)threadIdx.x) + (k & 3);
+            if (q < m) s_st[atomicAdd(&s_fill[key[k] >> W], 1u)] = make_uint2(key[k], (uint32_t)(s0 + q));
         }
         __syncthreads();
         for (int q = threadIdx.x; q < m; q += 256) {
@@ -445,8 +472,7 @@ __global__ void __launch_bounds__(256, 2) k_part_scatter(const int32_t* __restri
             pairs[s_cur[p] + (uint32_t)q - s_off[p]] = pr;
         }
         __syncthreads();
-        for (int p = threadIdx.x; p < P; p += 256) s_cur[p] += (p + 1 < PART_MAX ? s_off[p + 1] : (uint32_t)m) - s_off[p];
-        __syncthreads();
+        for (int p = threadIdx.x; p < P; p += 256) s_cur[p] += s_fill[p] - s_off[p];   // same p -> thread map as the clear
     }
 }
 
