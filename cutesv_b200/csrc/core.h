@@ -1220,4 +1220,46 @@ CSV_HD int32_t gc_union_minus(const int32_t* a, int na, const int32_t* b, int nb
     return dr;
 }
 
+// ------------------------------------------------------------------------------------------
+// INS/DEL density filter of one genome partition of bp 256-bp buckets (kernels.cuh k_part_filter).  Bucket b is kept
+// when it holds a signature and the buckets [b - rb, b + rb] hold >= need signatures; outside [0, bp) the window reads
+// the halo: hl[j] = signatures in the (j + 1)-th last bucket of the previous partition, hr[j] = in bucket j of the next
+// one (j < rb <= 64, zero where there is no neighbour).  h(b) is the count of bucket b in [0, bp).  A thread owns the
+// strip [b0, b0 + n) of n <= 64 consecutive buckets.
+// ------------------------------------------------------------------------------------------
+template <class H>
+CSV_HD uint32_t pf_count(const H& h, int k, int bp, const uint32_t* hl, const uint32_t* hr) {
+    return k < 0 ? hl[-k - 1] : k >= bp ? hr[k - bp] : h(k);
+}
+
+// Keep flags of a strip (bit j: bucket b0 + j) by a sliding window sum: 2 * rb + 1 reads for the first bucket, two for
+// every later one.  *kept = signatures in the strip's kept buckets.
+template <class H>
+CSV_HD uint64_t pf_strip_flags(const H& h, int b0, int n, int bp, int rb, uint32_t need, const uint32_t* hl, const uint32_t* hr,
+                               uint32_t* kept) {
+    uint32_t win = 0, sum = 0;
+    for (int k = b0 - rb; k <= b0 + rb; k++) win += pf_count(h, k, bp, hl, hr);
+    uint64_t flags = 0;
+    for (int j = 0; j < n; j++) {
+        const int b = b0 + j;
+        if (j) win += pf_count(h, b + rb, bp, hl, hr) - pf_count(h, b - rb - 1, bp, hl, hr);
+        const uint32_t c = h(b);
+        if (c > 0 && win >= need) { flags |= 1ull << j; sum += c; }
+    }
+    *kept = sum;
+    return flags;
+}
+
+// Exclusive offsets of a strip's kept buckets, the first at `base`: put(j, offset, kept, count) for every bucket of the
+// strip in order (count 0 for a dropped bucket, whose offset is that of the next kept one).
+template <class H, class F>
+CSV_HD void pf_strip_offsets(const H& h, int b0, int n, uint64_t flags, uint32_t base, F put) {
+    for (int j = 0; j < n; j++) {
+        const bool f = (flags >> j) & 1u;
+        const uint32_t c = f ? h(b0 + j) : 0u;
+        put(j, base, f, c);
+        base += c;
+    }
+}
+
 }  // namespace csv

@@ -37,17 +37,18 @@ __device__ __forceinline__ void lb_store(uint64_t* p, uint64_t v) {
 }
 __device__ __forceinline__ bool lb_ready(uint64_t v, uint32_t gen) { return (uint32_t)(v >> 32) == gen && (((uint32_t)v) >> 30) != 0; }
 
-// Warp-cooperative look-back (all 32 lanes of ONE warp call it): publishes `local` for `tile`
-// and returns the exclusive prefix over tiles < tile to every lane.  32 predecessors are
-// inspected per step, so a wave of W concurrently running tiles costs W/32 dependent L2 round
-// trips instead of W.
-__device__ __forceinline__ uint32_t lookback_exclusive_warp(uint64_t* status, uint32_t gen, int tile, uint32_t local) {
+// Publishes `local` for `tile` (one thread calls it); lookback_wait_warp later returns the tile's exclusive prefix.
+// Splitting the two lets a CTA do other work while its predecessors publish.
+__device__ __forceinline__ void lookback_publish(uint64_t* status, uint32_t gen, int tile, uint32_t local) {
+    lb_store(status + tile, lb_word(gen, local | (tile == 0 ? LB_INCL : LB_LOCAL)));
+}
+
+// Warp-cooperative wait (all 32 lanes of ONE warp call it) after lookback_publish(status, gen, tile, local): returns
+// the exclusive prefix over tiles < tile to every lane.  32 predecessors are inspected per step, so a wave of W
+// concurrently running tiles costs W/32 dependent L2 round trips instead of W.
+__device__ __forceinline__ uint32_t lookback_wait_warp(uint64_t* status, uint32_t gen, int tile, uint32_t local) {
     const int lane = threadIdx.x & 31;
-    if (tile == 0) {
-        if (lane == 0) lb_store(status, lb_word(gen, local | LB_INCL));
-        return 0;
-    }
-    if (lane == 0) lb_store(status + tile, lb_word(gen, local | LB_LOCAL));
+    if (tile == 0) return 0;
     uint32_t excl = 0;
     int p = tile - 1;
     while (true) {
@@ -70,6 +71,12 @@ __device__ __forceinline__ uint32_t lookback_exclusive_warp(uint64_t* status, ui
     }
     if (lane == 0) lb_store(status + tile, lb_word(gen, (excl + local) | LB_INCL));
     return excl;
+}
+
+// Both at once: publishes `local` for `tile` and returns its exclusive prefix (all 32 lanes of ONE warp call it).
+__device__ __forceinline__ uint32_t lookback_exclusive_warp(uint64_t* status, uint32_t gen, int tile, uint32_t local) {
+    if ((threadIdx.x & 31) == 0) lookback_publish(status, gen, tile, local);
+    return lookback_wait_warp(status, gen, tile, local);
 }
 
 // exclusive scan of one value per thread across a 256-thread CTA; returns exclusive prefix,

@@ -477,50 +477,50 @@ __global__ void __launch_bounds__(256) k_part_scatter(const int32_t* __restrict_
 }
 
 // One partition per CTA iteration (partitions taken by ticket, in order):
-//   1. 256-bp bucket histogram of the partition in shared memory, turned into an inclusive prefix (warp w owns the w-th
-//      eighth of the buckets; pre(i) adds the warp bases)
-//   2. flag of every bucket: the +-rb bucket window holds >= need signatures, the halo taken from the neighbours' edge
-//      counts -- the same rule as a genome-wide histogram; survivor total published to the look-back at once
-//   3. exclusive offsets of the flagged buckets, in place; the pairs are streamed again and every survivor is put into
-//      its bucket's slot range in the shared-memory stage (more than PF_STAGE survivors: in `spill`, at the output's offsets)
+//   1. 256-bp bucket histogram of the partition in shared memory
+//   2. one pass over every thread's strip of BP / 256 consecutive buckets: keep flags by a sliding +-rb window (the halo
+//      taken from the neighbours' edge counts -- the same rule as a genome-wide histogram) and the strip's survivors;
+//      one CTA scan gives the partition's survivor total, published to the look-back at once, and every strip's base
+//   3. a second pass over the strip writes the exclusive offsets of the kept buckets and their flag bits; the pairs are
+//      streamed again and every survivor is put into its bucket's slot range in the shared-memory stage (more than
+//      PF_STAGE survivors: in `spill`, at the output's offsets)
 //   4. order inside every bucket: rank against the bucket (<= FIX_SMALL members), or a CTA counting sort on the low
 //      BKT_SHIFT bits for larger buckets -> keys_out / idx_out at the partition's survivor base
+// Bucket b is stored transposed, at phys(b) = (b % per) * 256 + b / per (per = BP / 256 buckets per strip), so the 256
+// threads reading the j-th bucket of their strips touch 256 consecutive words.  The look-back's exclusive base is
+// awaited only where it is used: before the placement of a partition that spills, otherwise by warp 0 before its share
+// of the placement, while the other warps place theirs.
 __global__ void __launch_bounds__(256) k_part_filter(const uint2* __restrict__ pairs, const uint32_t* __restrict__ base, int P, int W, int rb,
                                                      uint32_t need, const uint32_t* __restrict__ edge, uint32_t* __restrict__ keys_out,
                                                      uint32_t* __restrict__ idx_out, uint2* __restrict__ spill, uint32_t* n_out, TileSync ts) {
     pdl_launch_dependents(); pdl_wait();
     extern __shared__ __align__(16) uint32_t s_dyn[];
-    const int BP = 1 << (W - BKT_SHIFT), WSH = W - BKT_SHIFT - 3, BPW = 1 << WSH;   // BPW buckets per warp
-    uint32_t* s_h = s_dyn;                                        // BP words
-    uint32_t* s_f = s_dyn + BP;                                   // BP / 32 flag words
+    const int BP = 1 << (W - BKT_SHIFT), LPER = W - BKT_SHIFT - 8, PER = 1 << LPER;   // PER buckets per strip
+    uint32_t* s_h = s_dyn;                                        // BP words, bucket b at phys(b)
+    uint32_t* s_f = s_dyn + BP;                                   // BP / 32 flag words, bit phys(b) % 32 of word phys(b) / 32
     uint2* s_st = reinterpret_cast<uint2*>(s_dyn + BP + BP / 32); // PF_STAGE pairs
-    __shared__ uint32_t s_warp[9], s_wb[9], s_fb[9];
-    __shared__ uint32_t s_hl[BKT_PAD + 1], s_hr[BKT_PAD + 1];
+    __shared__ uint32_t s_warp[9];
+    __shared__ uint32_t s_hl[BKT_PAD], s_hr[BKT_PAD];
     __shared__ uint32_t s_big[PF_BIG_CAP], s_cnt[256];
     __shared__ uint32_t s_tile, s_excl, s_nbig;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t gen = ts_gen(ts);
     const uint32_t bmask = BP - 1;
+    static_assert(PART_W_MIN - BKT_SHIFT >= 8 && PART_W_MAX - BKT_SHIFT <= 14, "one strip of 1..64 buckets per thread");
+    auto phys = [&](uint32_t b) -> uint32_t { return ((b & (PER - 1)) << 8) | (b >> LPER); };
+    auto count = [&](int b) -> uint32_t { return s_h[phys(b)]; };
+    const int b0 = (int)threadIdx.x * PER;   // this thread's strip
     while (true) {
         if (threadIdx.x == 0) { s_tile = atomicAdd(ts.ticket, 1u); s_nbig = 0; }
         for (int i = threadIdx.x; i < BP; i += 256) s_h[i] = 0;
         __syncthreads();
         const int p = (int)s_tile;
         if (p >= P) break;
-        if (warp < 2) {   // halo prefixes: s_hl[k] = the k last buckets of p-1, s_hr[k] = the k first buckets of p+1
-            const int q = warp == 0 ? p - 1 : p + 1;
-            const uint32_t* e = edge + (int64_t)q * 2 * BKT_PAD + (warp == 0 ? BKT_PAD : 0);
-            const bool ok = q >= 0 && q < P;
-            uint32_t v0 = ok && lane < rb ? e[lane] : 0u, v1 = ok && lane + 32 < rb ? e[lane + 32] : 0u;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) {
-                const uint32_t y0 = __shfl_up_sync(0xffffffffu, v0, d), y1 = __shfl_up_sync(0xffffffffu, v1, d);
-                if (lane >= d) { v0 += y0; v1 += y1; }
-            }
-            v1 += __shfl_sync(0xffffffffu, v0, 31);
-            uint32_t* h = warp == 0 ? s_hl : s_hr;
-            h[lane + 1] = v0; h[lane + 33] = v1;
-            if (lane == 0) h[0] = 0;
+        if (threadIdx.x < 2 * BKT_PAD) {   // halo: s_hl[j] = the (j+1)-th last bucket of p-1, s_hr[j] = bucket j of p+1
+            const int j = threadIdx.x % BKT_PAD, right = threadIdx.x / BKT_PAD;
+            const int q = right ? p + 1 : p - 1;
+            const bool ok = q >= 0 && q < P && j < rb;
+            (right ? s_hr : s_hl)[j] = ok ? edge[(int64_t)q * 2 * BKT_PAD + (right ? 0 : BKT_PAD) + j] : 0u;
         }
         const int64_t lo = base[p], cnt = (int64_t)base[p + 1] - lo;
         const uint2* src_pairs = pairs + lo;
@@ -532,97 +532,56 @@ __global__ void __launch_bounds__(256) k_part_filter(const uint2* __restrict__ p
             for (int u = 0; u < U; u++) k[u] = i0 + u * 256 < cnt ? src_pairs[i0 + u * 256].x : 0u;
 #pragma unroll
             for (int u = 0; u < U; u++)
-                if (i0 + u * 256 < cnt) atomicAdd(&s_h[(k[u] >> BKT_SHIFT) & bmask], 1u);
+                if (i0 + u * 256 < cnt) atomicAdd(&s_h[phys((k[u] >> BKT_SHIFT) & bmask)], 1u);
         }
         __syncthreads();
-        {   // inclusive prefix inside every warp's range
-            uint32_t run = 0;
-            for (int b = warp * BPW + lane; b < (warp + 1) * BPW; b += 32) {
-                uint32_t v = s_h[b];
-#pragma unroll
-                for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, v, d); if (lane >= d) v += y; }
-                s_h[b] = run + v;
-                run += __shfl_sync(0xffffffffu, v, 31);
-            }
-            if (lane == 0) s_warp[warp] = run;
-        }
-        __syncthreads();
+        // 2. keep flags of the strip, the partition's survivor total and the strip's first slot
+        uint32_t kept, S;
+        const uint64_t flags = pf_strip_flags(count, b0, PER, BP, rb, need, s_hl, s_hr, &kept);
+        const uint32_t first = block_excl_scan_256(kept, s_warp, &S);
         if (threadIdx.x == 0) {
-            uint32_t r = 0;
-            for (int w = 0; w < 8; w++) { s_wb[w] = r; r += s_warp[w]; }
-            s_wb[8] = r;
+            lookback_publish(ts.status, gen, p, S);
+            if (S) atomicAdd(n_out, S);
         }
-        __syncthreads();
-        auto pre = [&](int i) -> uint32_t { return i < 0 ? 0u : s_h[i] + s_wb[i >> WSH]; };   // buckets [0, i]
-        // 2. flags and the survivors of every warp's range
-        {
-            uint32_t mine = 0;
-            for (int b = warp * BPW + lane; b < (warp + 1) * BPW; b += 32) {
-                const uint32_t c = pre(b) - pre(b - 1);
-                uint32_t win = pre(min(b + rb, BP - 1)) - pre(b - rb - 1);
-                if (b < rb) win += s_hl[rb - b];
-                if (b + rb >= BP) win += s_hr[b + rb - BP + 1];
-                const bool f = c > 0 && win >= need;
-                const uint32_t bits = __ballot_sync(0xffffffffu, f);
-                if (lane == 0) s_f[b >> 5] = bits;
-                if (f) mine += c;
-            }
-#pragma unroll
-            for (int d = 16; d > 0; d >>= 1) mine += __shfl_xor_sync(0xffffffffu, mine, d);
-            if (lane == 0) s_warp[warp] = mine;
-        }
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            uint32_t r = 0;
-            for (int w = 0; w < 8; w++) { s_fb[w] = r; r += s_warp[w]; }
-            s_fb[8] = r;
-        }
-        __syncthreads();
-        const uint32_t S = s_fb[8];
-        if (warp == 0) {   // publish the partition's survivor count at once, then wait for the base
-            const uint32_t ex = lookback_exclusive_warp(ts.status, gen, p, S);
-            if (lane == 0) { s_excl = ex; if (S) atomicAdd(n_out, S); }
-        }
-        {   // 3a. exclusive offsets of the flagged buckets, in place (a warp reads and writes only its own range)
-            uint32_t run = s_fb[warp], prev = s_wb[warp];
-            for (int b = warp * BPW + lane; b < (warp + 1) * BPW; b += 32) {
-                const uint32_t pb = s_h[b] + s_wb[warp];
-                uint32_t pm = __shfl_up_sync(0xffffffffu, pb, 1);
-                if (lane == 0) pm = prev;
-                prev = __shfl_sync(0xffffffffu, pb, 31);
-                const uint32_t c = ((s_f[b >> 5] >> lane) & 1u) ? pb - pm : 0u;
-                uint32_t v = c;
-#pragma unroll
-                for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, v, d); if (lane >= d) v += y; }
-                s_h[b] = run + v - c;
-                run += __shfl_sync(0xffffffffu, v, 31);
-                if (c > FIX_SMALL) {
-                    const uint32_t q = atomicAdd(&s_nbig, 1u);
-                    if (q < PF_BIG_CAP) s_big[q] = b;
-                }
-            }
-        }
-        __syncthreads();
-        const uint32_t obase = s_excl;
         const bool spilled = S > (uint32_t)PF_STAGE;
-        uint2* st = spilled ? spill + obase : s_st;
-        // 3b. survivors into their buckets' slot ranges (afterwards s_h[b] = end of bucket b)
+        if (spilled && warp == 0) {   // the spill area lies at the partition's output offsets
+            const uint32_t ex = lookback_wait_warp(ts.status, gen, p, S);
+            if (lane == 0) s_excl = ex;
+        }
+        // 3a. exclusive offsets of the kept buckets in place, their flag bits, the list of large buckets
+        pf_strip_offsets(count, b0, PER, flags, first, [&](int j, uint32_t off, bool f, uint32_t c) {
+            s_h[(j << 8) | threadIdx.x] = off;   // phys(b0 + j)
+            const uint32_t bits = __ballot_sync(0xffffffffu, f);
+            if (lane == 0) s_f[(j << 3) | warp] = bits;
+            if (c > FIX_SMALL) {
+                const uint32_t q = atomicAdd(&s_nbig, 1u);
+                if (q < PF_BIG_CAP) s_big[q] = (uint32_t)(b0 + j);
+            }
+        });
+        __syncthreads();
+        if (!spilled && warp == 0) {   // the other warps start placing meanwhile
+            const uint32_t ex = lookback_wait_warp(ts.status, gen, p, S);
+            if (lane == 0) s_excl = ex;
+        }
+        uint2* st = spilled ? spill + s_excl : s_st;
+        // 3b. survivors into their buckets' slot ranges (afterwards s_h[phys(b)] = end of bucket b)
         for (int64_t i0 = threadIdx.x; i0 < cnt; i0 += 256 * U) {
             uint2 pr[U];
 #pragma unroll
             for (int u = 0; u < U; u++) pr[u] = i0 + u * 256 < cnt ? src_pairs[i0 + u * 256] : make_uint2(0u, 0u);
 #pragma unroll
             for (int u = 0; u < U; u++) {
-                const uint32_t b = (pr[u].x >> BKT_SHIFT) & bmask;
-                if (i0 + u * 256 < cnt && ((s_f[b >> 5] >> (b & 31)) & 1u)) st[atomicAdd(&s_h[b], 1u)] = pr[u];
+                const uint32_t ph = phys((pr[u].x >> BKT_SHIFT) & bmask);
+                if (i0 + u * 256 < cnt && ((s_f[ph >> 5] >> (ph & 31)) & 1u)) st[atomicAdd(&s_h[ph], 1u)] = pr[u];
             }
         }
         __syncthreads();
+        const uint32_t obase = s_excl;
         // 4a. small buckets: rank against the bucket, ties by slot
         for (uint32_t q = threadIdx.x; q < S; q += 256) {
             const uint2 pr = st[q];
             const uint32_t b = (pr.x >> BKT_SHIFT) & bmask;
-            const uint32_t beg = b ? s_h[b - 1] : 0u, end = s_h[b];
+            const uint32_t beg = b ? s_h[phys(b - 1)] : 0u, end = s_h[phys(b)];
             if (end - beg > FIX_SMALL) continue;
             uint32_t rank = 0;
             for (uint32_t j = beg; j < end; j++) {
@@ -638,7 +597,7 @@ __global__ void __launch_bounds__(256) k_part_filter(const uint2* __restrict__ p
         const uint32_t nb = nbig <= (uint32_t)PF_BIG_CAP ? nbig : (uint32_t)BP;   // list overflow: visit every bucket
         for (uint32_t k = 0; k < nb; k++) {
             const uint32_t b = nbig <= (uint32_t)PF_BIG_CAP ? s_big[k] : k;
-            const uint32_t beg = b ? s_h[b - 1] : 0u, end = s_h[b];
+            const uint32_t beg = b ? s_h[phys(b - 1)] : 0u, end = s_h[phys(b)];
             if (end - beg <= FIX_SMALL) continue;   // (uniform across the CTA)
             __syncthreads();
             s_cnt[threadIdx.x] = 0;
