@@ -2,7 +2,7 @@
 `Engine.extract` consumes, without a Python loop over reads (replaces the pysam iteration of
 cuteSV:709-733 and the per-read packing of packing.pack_alignments for plain BAM input).
 
-Sequential decode only; the .bai is read just for the per-contig mapped counts that size the task
+Sequential decode only; the .bai (or .csi) is read just for the per-contig mapped counts that size the task
 windows (get_index_statistics, cuteSV:1015-1025).
 """
 import ctypes as C
@@ -103,12 +103,13 @@ class BamReader(object):
         return self.lengths[self.references.index(name)]
 
     def index_statistics(self):
-        """[(contig, mapped)] in header order, like pysam's get_index_statistics()."""
-        bai = self.path + ".bai"
-        if not os.path.exists(bai):
-            bai = os.path.splitext(self.path)[0] + ".bai"
+        """[(contig, mapped)] in header order, like pysam's get_index_statistics().  Reads <bam>.bai or <stem>.bai, else the
+        CSI index <bam>.csi or <stem>.csi (`samtools index -c`, which contigs longer than 2^29 bp need)."""
+        stem = os.path.splitext(self.path)[0]
+        cands = [self.path + ".bai", stem + ".bai", self.path + ".csi", stem + ".csi"]
+        idx = next((p for p in cands if os.path.exists(p)), cands[1])
         mapped = np.zeros(max(len(self.references), 1), dtype=np.int64)
-        if lib().bamr_index_stats(os.fsencode(bai), len(self.references), mapped.ctypes.data_as(_I64P)) != 0:
+        if lib().bamr_index_stats(os.fsencode(idx), len(self.references), mapped.ctypes.data_as(_I64P)) != 0:
             raise IOError(lib().bamr_error().decode())
         return [(n, int(mapped[i])) for i, n in enumerate(self.references)]
 

@@ -107,11 +107,17 @@ def load_bed(bed_file, tasks):
             s = line.strip().split("\t")
             regions.setdefault(s[0], []).append((int(s[1]) - 1000, int(s[2]) + 1000))
     out = [[] for _ in tasks]
+    # the reference scans every task for every region; only the tasks of the region's own contig can match, so visiting
+    # just those (in task order) gives the same lists in the same order without O(regions x tasks) on many-contig genomes
+    by_contig = {}
+    for i, t in enumerate(tasks):
+        by_contig.setdefault(t[0], []).append(i)
     for chrom in regions:
         regions[chrom].sort()
+        own = [(i, tasks[i]) for i in by_contig.get(chrom, ())]
         for item in regions[chrom]:
-            for i, t in enumerate(tasks):
-                if chrom == t[0] and ((t[1] <= item[0] and t[2] > item[0]) or item[0] <= t[1] < item[1]):
+            for i, t in own:
+                if (t[1] <= item[0] and t[2] > item[0]) or item[0] <= t[1] < item[1]:
                     out[i].append(item)
     return out
 

@@ -587,13 +587,61 @@ void bamr_unpack_ranges(const uint8_t* seq4, int64_t n, const int64_t* nib0, con
     }
 }
 
+// The same counts from a CSI index (`samtools index -c`, needed for contigs longer than 2^29 bp). The file is BGZF
+// compressed: magic, min_shift, depth, l_aux, aux, n_ref; per reference n_bin bins of (bin, loffset, n_chunk, chunks) and
+// no linear index. The pseudo-bin is ((1 << 3*(depth+1)) - 1)/7 + 1; its second chunk holds (n_mapped, n_unmapped).
+static int csi_stats(const char* path, int32_t n_ref, int64_t* mapped) {
+    gzFile f = gzopen(path, "rb");
+    if (!f) { g_err = std::string("cannot open ") + path; return -1; }
+    std::vector<uint8_t> d;
+    std::vector<uint8_t> buf(1 << 16);
+    int k;
+    while ((k = gzread(f, buf.data(), (unsigned)buf.size())) > 0) d.insert(d.end(), buf.begin(), buf.begin() + k);
+    int zerr = Z_OK;
+    gzerror(f, &zerr);
+    gzclose(f);
+    if (k < 0 || (zerr != Z_OK && zerr != Z_STREAM_END)) { g_err = "truncated or corrupt CSI (BGZF decompression failed)"; return -1; }
+    size_t p = 0;
+    auto have = [&](uint64_t b) { return b <= d.size() - p; };
+    if (!have(16) || memcmp(d.data(), "CSI\1", 4) != 0) { g_err = "not a CSI index"; return -1; }
+    const int32_t min_shift = rd_i32(d.data() + 4), depth = rd_i32(d.data() + 8), l_aux = rd_i32(d.data() + 12);
+    if (min_shift < 0 || depth < 0 || depth > 10) { g_err = "malformed CSI (min_shift / depth)"; return -1; }
+    p = 16;
+    if (l_aux < 0 || !have((uint64_t)l_aux + 4)) { g_err = "truncated CSI (header)"; return -1; }
+    p += (size_t)l_aux;
+    const int32_t n = rd_i32(d.data() + p);
+    p += 4;
+    if (n < 0) { g_err = "malformed CSI (negative reference count)"; return -1; }
+    const uint32_t pseudo = (uint32_t)((((uint64_t)1 << (3 * (depth + 1))) - 1) / 7 + 1);
+    for (int32_t i = 0; i < n_ref; i++) mapped[i] = 0;
+    for (int32_t ref = 0; ref < n; ref++) {
+        if (!have(4)) { g_err = "truncated CSI"; return -1; }
+        const int32_t n_bin = rd_i32(d.data() + p);
+        p += 4;
+        if (n_bin < 0) { g_err = "malformed CSI (negative bin count)"; return -1; }
+        for (int32_t b = 0; b < n_bin; b++) {
+            if (!have(16)) { g_err = "truncated CSI"; return -1; }
+            const uint32_t bin = rd_u32(d.data() + p);
+            const int32_t n_chunk = rd_i32(d.data() + p + 12);   // after bin (4 B) and loffset (8 B)
+            p += 16;
+            if (n_chunk < 0) { g_err = "malformed CSI (chunk count)"; return -1; }
+            if (!have((uint64_t)n_chunk * 16)) { g_err = "truncated CSI"; return -1; }
+            if (bin == pseudo && n_chunk >= 2 && ref < n_ref) { uint64_t m; memcpy(&m, d.data() + p + 16, 8); mapped[ref] = (int64_t)m; }
+            p += (size_t)n_chunk * 16;
+        }
+    }
+    return 0;
+}
+
 // Per-reference mapped-read counts from a .bai index (get_index_statistics, cuteSV:1015-1025):
-// the pseudo-bin 37450 of every reference holds (n_mapped, n_unmapped).
+// the pseudo-bin 37450 of every reference holds (n_mapped, n_unmapped).  A BGZF-compressed file is read as CSI.
 static int bamr_index_stats_impl(const char* bai_path, int32_t n_ref, int64_t* mapped) {
     FILE* f = fopen(bai_path, "rb");
     if (!f) { g_err = std::string("cannot open ") + bai_path; return -1; }
     uint8_t h[8];
-    if (fread(h, 1, 8, f) != 8 || memcmp(h, "BAI\1", 4) != 0) { fclose(f); g_err = "not a BAI index"; return -1; }
+    const size_t got = fread(h, 1, 8, f);
+    if (got >= 2 && h[0] == 31 && h[1] == 139) { fclose(f); return csi_stats(bai_path, n_ref, mapped); }
+    if (got != 8 || memcmp(h, "BAI\1", 4) != 0) { fclose(f); g_err = "not a BAI index"; return -1; }
     const int32_t n = rd_i32(h + 4);
     for (int32_t i = 0; i < n_ref; i++) mapped[i] = 0;
     for (int32_t ref = 0; ref < n; ref++) {

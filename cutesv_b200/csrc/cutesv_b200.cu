@@ -556,6 +556,8 @@ extern "C" int csv_set_params(csv_ctx* c, const csv_params* p) {
 
 extern "C" int csv_set_contigs(csv_ctx* c, int32_t n, const int64_t* lens) {
     if (!c || n < 1 || !lens) return set_err(CSV_E_INVALID, "bad contig table");
+    // TRA signatures and candidates carry chr2*4+type in int32
+    if (n >= (1 << 29)) return set_err(CSV_E_INVALID, "%d contigs: at most 2^29 - 1 are supported", n);
     CU(cudaSetDevice(c->device));
     if (c->off_pad == 0) csv_set_params(c, &c->P);
     if ((int32_t)c->owned.size() != n) c->owned.clear();   // a new table drops the shard mask
@@ -732,11 +734,10 @@ extern "C" int csv_upload_alignments(csv_ctx* c, const csv_reads_cols* h) {
     CU(c->aln_flag.ensure(64));
     uint32_t* flag = c->aln_flag.as<uint32_t>();
     CU(cudaMemsetAsync(flag, 0, 4, c->stream));
-    CU(cudaMemsetAsync(c->a_off.p, 0xff, ((size_t)c->n_contigs + 2) * 4, c->stream));
     CU(cudaMemsetAsync(c->a_span.p, 0, ((size_t)c->n_contigs + 2) * 4, c->stream));
     LAUNCH(c, k_aln_index, grid_for(c, h->n, 256), 256, 0, c->a_chrom.as<int32_t>(), c->a_start.as<int32_t>(), c->a_end.as<int32_t>(), h->n,
-           c->n_contigs, c->a_off.as<uint32_t>(), c->a_span.as<int32_t>(), flag);
-    LAUNCH(c, k_aln_fill, 1, 32, 0, c->a_off.as<uint32_t>(), c->n_contigs, (uint32_t)h->n);
+           c->n_contigs, c->a_span.as<int32_t>(), flag);
+    LAUNCH(c, k_aln_off, grid_for(c, (int64_t)c->n_contigs + 1, 256), 256, 0, c->a_chrom.as<int32_t>(), h->n, c->n_contigs, c->a_off.as<uint32_t>());
     uint32_t hflag = 0;
     CU(cudaMemcpyAsync(&hflag, flag, 4, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
@@ -1035,20 +1036,46 @@ static int run_other(csv_ctx* c, int t, uint32_t kslot_base) {
     SmallWork& w = c->small;
     ContigTab ct{c->d_off.as<uint64_t>(), c->d_len_eff.as<int64_t>(), c->n_contigs};
     Counters* ctr = c->counters.as<Counters>();
-    const int cb = bits_for((uint64_t)c->n_contigs);
-    if (t == CSV_TRA && cb > 15) return set_err(CSV_E_INVALID, "TRA: more than 32767 contigs are not supported");
     // primary key = (chr, a) | (chr, strand, a) | (chr1, chr2*4+type, a): value range sized from the contig count
     const uint64_t hi_max = t == CSV_DUP ? (uint64_t)c->n_contigs : t == CSV_INV ? 2ull * c->n_contigs : 4ull * c->n_contigs * c->n_contigs;
-    const int prim_bits = 31 + bits_for(hi_max);
+    // The packed TRA key needs 2*ceil(log2 n_contigs) + 33 bits.  On more than 32768 contigs (chr1, chr2*4+type) is
+    // replaced by its dense rank among the pairs present, which is below the signature count, so the key stays (rank, a)
+    // in 31 + bits_for(n) bits
+    const int clog = c->n_contigs > 1 ? bits_for((uint64_t)c->n_contigs - 1) : 0;   // ceil(log2 n_contigs)
+    const bool compact = t == CSV_TRA && 2 * clog + 33 > 64;
+    const int prim_bits = 31 + bits_for(compact ? (uint64_t)n : hi_max);
     const int32_t* col_c = s.has_c ? s.c.as<int32_t>() : nullptr;
     const bool chain = c->small_chain[t];
+    uint64_t* k_prim = chain ? w.k_prim.as<uint64_t>() : c->keys_a.as<uint64_t>();
+    int rc;
     stage_begin(c, CSV_ST_KEYS);
-    LAUNCH(c, k_other_keys, grid_for(c, n, 256), 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), s.b.as<int32_t>(), s.rid.as<int32_t>(),
-           col_c, n, t, ct, chain ? w.k_rid.as<uint32_t>() : (uint32_t*)nullptr, w.k_b.as<uint32_t>(),
-           chain ? w.k_prim.as<uint64_t>() : c->keys_a.as<uint64_t>(), &ctr->status);
+    if (!compact) {
+        LAUNCH(c, (k_other_keys<false>), grid_for(c, n, 256), 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), s.b.as<int32_t>(),
+               s.rid.as<int32_t>(), col_c, n, t, ct, chain ? w.k_rid.as<uint32_t>() : (uint32_t*)nullptr, w.k_b.as<uint32_t>(), k_prim,
+               &ctr->status);
+    } else {
+        // pair words -> sort -> flags at pair changes -> exclusive scan = ranks -> (rank, a) scattered back to input order
+        LAUNCH(c, (k_other_keys<true>), grid_for(c, n, 256), 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), s.b.as<int32_t>(),
+               s.rid.as<int32_t>(), col_c, n, t, ct, chain ? w.k_rid.as<uint32_t>() : (uint32_t*)nullptr, w.k_b.as<uint32_t>(),
+               c->keys_a.as<uint64_t>(), &ctr->status);
+        uint64_t* pair_sorted = nullptr;
+        uint32_t* pair_perm = nullptr;
+        rc = radix_sort<uint64_t>(c, c->keys_a.as<uint64_t>(), c->vals_a.as<uint32_t>(), c->keys_b.as<uint64_t>(), c->vals_b.as<uint32_t>(),
+                                  true, n, nullptr, bits_for(hi_max), &pair_sorted, &pair_perm);
+        if (rc) return rc;
+        uint32_t* rank = w.sel.as<uint32_t>();   // free until the de-duplication below
+        LAUNCH(c, k_tra_pair_flags, grid_for(c, n, 256), 256, 0, (const uint64_t*)pair_sorted, n, rank);
+        TileSync ts;
+        rc = make_sync(c, (size_t)(n / (SEL_THREADS * 4) + 2), &ts);
+        if (rc) return rc;
+        LAUNCH(c, (k_scan_excl<4>), grid_for(c, n, SEL_THREADS * 4, 4), SEL_THREADS, 0, rank, n, (const uint32_t*)nullptr,
+               (const uint32_t*)nullptr, (uint32_t*)nullptr, ts);
+        // k_prim may alias pair_sorted (keys_a), which is no longer read; pair_perm is a value buffer
+        LAUNCH(c, k_tra_compact_key, grid_for(c, n, 256), 256, 0, (const uint32_t*)pair_perm, (const uint32_t*)rank, s.a.as<int32_t>(), n,
+               k_prim);
+    }
     stage_end(c, CSV_ST_KEYS);
     stage_begin(c, CSV_ST_SORT);
-    int rc;
     if (!chain) {
         // ONE sort on the primary key (<= 8 passes instead of 16), then (b, name) order inside runs of equal primary keys
         uint64_t* k64o = nullptr;

@@ -620,6 +620,9 @@ __global__ void __launch_bounds__(256) k_part_filter(const uint2* __restrict__ p
 }
 
 // small types: three sort keys per signature (name, second coordinate, primary)
+// TRA_PAIR: k_prim receives only the TRA pair word chr1*4n + chr2*4+type, for contig counts at which the pair and pos1 do not
+// fit one 64-bit key; k_tra_compact_key then replaces it by (dense rank of the pair, pos1)
+template <bool TRA_PAIR>
 __global__ void k_other_keys(const int32_t* __restrict__ chrom, const int32_t* __restrict__ a, const int32_t* __restrict__ b,
                              const int32_t* __restrict__ rid, const int32_t* __restrict__ c, int64_t n, int svtype, ContigTab ct,
                              uint32_t* __restrict__ k_rid, uint32_t* __restrict__ k_b, uint64_t* __restrict__ k_prim,
@@ -638,7 +641,23 @@ __global__ void k_other_keys(const int32_t* __restrict__ chrom, const int32_t* _
         uint64_t hi = (uint64_t)(uint32_t)ch;
         if (svtype == CSV_INV) hi = hi * 2 + (uint32_t)ci;
         if (svtype == CSV_TRA) hi = hi * (uint64_t)(4 * ct.n) + (uint32_t)ci;   // chr2*4+type < 4*n_contigs
-        k_prim[i] = (hi << 31) | (uint32_t)ai;                     // a < 2^31
+        k_prim[i] = TRA_PAIR ? hi : (hi << 31) | (uint32_t)ai;     // a < 2^31
+    }
+}
+
+// flag[i] = 1 where the sorted TRA pair word changes after position i: the exclusive scan of the flags is the dense rank
+// of pair[i] among the pairs present
+__global__ void k_tra_pair_flags(const uint64_t* __restrict__ pair_sorted, int64_t n, uint32_t* __restrict__ flag) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+        flag[i] = (i + 1 < n && pair_sorted[i + 1] != pair_sorted[i]) ? 1u : 0u;
+}
+// compact TRA primary key in input order: (rank of (chr1, chr2*4+type), pos1).  Ranks keep the pairs' order, so the key
+// sorts, ties and runs exactly as (chr1, chr2*4+type, pos1) does.
+__global__ void k_tra_compact_key(const uint32_t* __restrict__ perm, const uint32_t* __restrict__ rank, const int32_t* __restrict__ a,
+                                  int64_t n, uint64_t* __restrict__ k_prim) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const uint32_t x = perm[i];
+        k_prim[x] = ((uint64_t)rank[i] << 31) | (uint32_t)a[x];
     }
 }
 
@@ -1329,20 +1348,24 @@ __global__ void k_finalize(GenoJob G) {
 
 // ---- TRA genotyping from the packed all-alignments table ----
 __global__ void k_aln_index(const int32_t* __restrict__ chrom, const int32_t* __restrict__ start, const int32_t* __restrict__ end, int64_t n,
-                            int32_t n_contigs, uint32_t* off, int32_t* max_span, uint32_t* status) {
+                            int32_t n_contigs, int32_t* max_span, uint32_t* status) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         const int32_t c = chrom[i];
         if (c < 0 || c >= n_contigs) { atomicOr(status, ST_BAD_CHROM); continue; }
-        if (i == 0 || chrom[i - 1] != c) off[c] = (uint32_t)i;
         if (i > 0 && (chrom[i - 1] > c || (chrom[i - 1] == c && start[i - 1] > start[i]))) atomicOr(status, ST_UNSORTED);
         atomicMax(&max_span[c], end[i] - start[i]);
     }
 }
-__global__ void k_aln_fill(uint32_t* off, int32_t n_contigs, uint32_t n) {
-    if (blockIdx.x == 0 && threadIdx.x == 0) {
-        off[n_contigs] = n;
-        for (int c = n_contigs - 1; c >= 0; c--)
-            if (off[c] == 0xffffffffu) off[c] = off[c + 1];
+// off[c] = first row of contig c, i.e. the lower bound of c in the contig-sorted column, for c in [0, n_contigs]:
+// one thread per contig (k_aln_index rejects a column that is not sorted)
+__global__ void k_aln_off(const int32_t* __restrict__ chrom, int64_t n, int32_t n_contigs, uint32_t* __restrict__ off) {
+    for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c <= n_contigs; c += (int64_t)gridDim.x * blockDim.x) {
+        int64_t lo = 0, hi = n;
+        while (lo < hi) {
+            const int64_t mid = (lo + hi) >> 1;
+            if (chrom[mid] < c) lo = mid + 1; else hi = mid;
+        }
+        off[c] = (uint32_t)lo;
     }
 }
 // Warp-cooperative count_coverage (core.h tra_count_coverage is the scalar statement the emulator runs):

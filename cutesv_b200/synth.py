@@ -626,6 +626,120 @@ def synth_bam_dataset(seed=1, n_contigs=2, contig_len=120000, coverage=22, read_
     return dict(contigs=[(nm, contig_len) for nm in names], reads=reads), fasta
 
 
+def draft_names(n):
+    """Scaffold names of a draft assembly in header order: unpadded numbers, so string order differs from numeric order."""
+    return ["scaffold_%d" % k for k in range(n)]
+
+
+def draft_assembly(n_contigs, seed=7, n_active=40, active_len=400000, n_reads=6000, scale=1.0, median_len=30000.0):
+    """Columnar inputs (like make_config) on a draft assembly of `n_contigs` scaffolds with lognormal lengths (median
+    `median_len`, at least 1000 bp; the active scaffolds at least `active_len`).  Reads and
+    signatures of all five types sit on `n_active` scaffolds that include the contig ids 0, 32767, 32768 and n-1 (those that
+    exist); TRA mates pair them up.  Contig ids are ranks of the names in string order, as the C-ABI requires."""
+    rng = np.random.default_rng(seed)
+    header = draft_names(n_contigs)
+    by_name = sorted(range(n_contigs), key=header.__getitem__)   # contig id (string-order rank) -> header index
+    lens = np.clip(rng.lognormal(np.log(median_len), 1.2, n_contigs), 1000, 5000000).astype(np.int64)[by_name]
+    want = [i for i in (0, 32767, 32768, n_contigs - 1) if 0 <= i < n_contigs]
+    pool = np.setdiff1d(np.arange(n_contigs), want)
+    act = np.unique(np.concatenate([want, rng.choice(pool, min(len(pool), max(n_active - len(want), 0)), replace=False)])).astype(np.int32)
+    lens[act] = np.maximum(lens[act], active_len)
+    la = lens[act]
+    reads = synth_reads(rng, la, n_reads, normal=(18000.0, 3000.0), lo=1000, hi=60000)
+    sigs = {"DEL": synth_indel(rng, la, reads, int(40000 * scale), int(600 * scale), "DEL"),
+            "INS": synth_indel(rng, la, reads, int(40000 * scale), int(600 * scale), "INS"),
+            "DUP": synth_dup(rng, la, reads, int(300 * scale), int(2000 * scale)),
+            "INV": synth_inv(rng, la, reads, int(100 * scale), int(1000 * scale)),
+            "TRA": synth_tra(rng, la, reads, int(300 * scale), int(3000 * scale))}
+    reads["chrom"] = act[reads["chrom"]]
+    for t, s in sigs.items():
+        s["chrom"] = act[s["chrom"]]
+        if t == "TRA":
+            s["c"] = (act[s["c"] >> 2] * 4 + (s["c"] & 3)).astype(np.int32)
+    params = dict(min_support=3, bias_ins=1000, ratio_ins=0.9, bias_del=1000, ratio_del=0.5, genotype=1)
+    names = [header[k] for k in by_name]
+    return dict(names=names, lens=lens, reads=reads, sigs=sigs, params=params, active=act,
+                n_sigs=int(sum(len(v["chrom"]) for v in sigs.values())))
+
+
+def synth_draft_bam_dataset(seed=11, n_header=40000, n_active=30, contig_len=60000, coverage=14, read_len=(2500, 7000)):
+    """Like synth_bam_dataset on a draft assembly: `n_header` scaffolds in the BAM header, reads on `n_active` of them (among
+    them scaffolds whose string-order rank is above 32767), DEL / INS loci in the CIGARs and TRA loci as split reads whose
+    SA mate lies on another active scaffold.  Returns dict(contigs=[(name, len)], reads=[SynthRead]), fasta of the active
+    scaffolds {name: seq}."""
+    rng = np.random.default_rng(seed)
+    names = draft_names(n_header)
+    rank = {n: i for i, n in enumerate(sorted(names))}
+    lens = np.clip(rng.lognormal(np.log(3000.0), 0.8, n_header), 500, 40000).astype(np.int64)
+    hi_rank = [k for k in range(n_header) if rank[names[k]] > 32767]
+    act = sorted(set(rng.choice(n_header, n_active // 2, replace=False).tolist()) | set(rng.choice(hi_rank, n_active - n_active // 2, replace=False).tolist()))
+    for k in act:
+        lens[k] = contig_len
+    loci = {}
+    for k in act:
+        pos, lk = 6000, []
+        while pos < contig_len - 8000:
+            kind = str(rng.choice(["DEL", "INS", "DEL", "INS", "TRA"]))
+            mate = int(rng.choice([j for j in act if j != k]))
+            lk.append((int(pos), kind, int(rng.integers(60, 600)), bool(rng.random() < 0.5), mate))
+            pos += int(rng.integers(5000, 9000))
+        loci[k] = lk
+    reads, rid = [], 0
+    for k in act:
+        nm = names[k]
+        n_reads = int(coverage * contig_len / ((read_len[0] + read_len[1]) / 2))
+        for st in np.sort(rng.integers(0, contig_len - read_len[1] - 1000, n_reads)):
+            L = int(rng.integers(read_len[0], read_len[1]))
+            r = SynthRead()
+            r.query_name = read_name(rid)
+            rid += 1
+            r.flag = 0 if rng.random() < 0.5 else 16
+            r.mapq = int(rng.choice([60, 60, 60, 30, 10]))
+            r.reference_name = nm
+            r.reference_start = int(st)
+            ops, ref, end, tags, tra_hit = [], int(st), int(st) + L, [("NM", 5)], None
+            for (lp, kind, ln, hom, mate) in loci[k]:
+                if not (ref + 300 < lp < end - 300) or (not hom and rng.random() < 0.5):
+                    continue
+                if kind == "TRA":
+                    tra_hit = (lp, ln, mate)
+                    break
+                lp2 = lp + int(rng.integers(-8, 9))
+                if lp2 <= ref + 20:
+                    continue
+                ops.append((0, lp2 - ref))
+                ref = lp2
+                ln2 = max(int(ln * rng.normal(1.0, 0.03)), 30)
+                if kind == "DEL":
+                    ops.append((2, ln2))
+                    ref += ln2
+                else:
+                    ops.append((1, ln2))
+            if tra_hit is not None:
+                end = max(tra_hit[0] + int(rng.integers(-5, 6)), ref + 1)
+            if end > ref:
+                ops.append((0, end - ref))
+                ref = end
+            clip = 0
+            if tra_hit is not None:   # split read: the tail maps to the locus' mate scaffold
+                clip = int(rng.integers(800, 2000))
+                ops.append((4, clip))
+            qlen = sum(l for o, l in ops if o in (0, 1, 4, 7, 8))
+            if tra_hit is not None:
+                tgt = 20000 + tra_hit[1] * 10 + int(rng.integers(-5, 6))
+                tags.append(("SA", "%s,%d,+,%dS%dM,60,3;" % (names[tra_hit[2]], tgt, qlen - clip, clip)))
+                r.flag = 0
+            r.cigartuples = ops
+            r.cigar = ops
+            r.query_length = qlen
+            r.reference_end = ref
+            r.query_sequence = "".join(rng.choice(list("ACGT"), qlen))
+            r.tags = tags
+            reads.append(r)
+    fasta = {names[k]: "".join(rng.choice(list("ACGT"), contig_len + 10)) for k in act}
+    return dict(contigs=[(names[k], int(lens[k])) for k in range(n_header)], reads=reads), fasta
+
+
 def synth_cigar_packet(n_reads, mean_indels=850, seed=5, n_contigs=25, sa_frac=0.0):
     """Vectorised packed alignment packet (no Python objects) shaped like ONT reads: ~1 CIGAR op per
     7 bp, M / small indel alternation, ~1 qualifying (>= 10 bp) insertion and deletion per read

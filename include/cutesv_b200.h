@@ -162,7 +162,11 @@ int csv_create(int device, void* stream, csv_ctx** out);
 int csv_destroy(csv_ctx* ctx);
 int csv_set_params(csv_ctx* ctx, const csv_params* p);
 /* Contig table: id = rank of the name in Python string order; lens from the BAM header
- * (cuteSV:1029).  Needed to linearise (contig, pos) into one sortable coordinate. */
+ * (cuteSV:1029).  Needed to linearise (contig, pos) into one sortable coordinate.  Up to 2^29 - 1
+ * contigs (draft assemblies with 10^5-10^6 scaffolds included; TRA's chr2*4+type is int32); more are
+ * CSV_E_INVALID.  Every contig must be shorter than 2^30 bp, since INS positions and genotype windows
+ * are half units in int32.  That length limit is NOT validated here: lengths up to 2^31 - 1 are
+ * accepted, and INS / genotyping results on a contig of 2^30 bp or more are undefined. */
 int csv_set_contigs(csv_ctx* ctx, int32_t n_contigs, const int64_t* contig_len);
 
 /* Pinned host memory helpers (caller-owned buffers stay caller-owned). */
@@ -188,6 +192,8 @@ int csv_upload_reads_grouped(csv_ctx* ctx, const csv_reads_cols* host_cols, cons
  * The reference re-opens the BAM per TRA candidate and iterates bam.fetch() with an early exit
  * (call_gt resolveTRA.py:260-309, count_coverage cuteSV_genotype.py:72-93); with this table the same
  * scan runs on the device.  Without it TRA rows keep CSV_F_GT_HOST.  n == 0 clears the table.
+ * The per-contig row index is built in parallel (one thread per contig), so the call stays cheap at
+ * large contig counts.
  * Precondition (as for the reads table): one primary record per read name. */
 int csv_upload_alignments(csv_ctx* ctx, const csv_reads_cols* aln);
 
