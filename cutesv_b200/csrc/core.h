@@ -765,26 +765,29 @@ CSV_HD void indel_cluster(Team tm, const IndelView& in, int64_t s, int m, int M,
         }
         const double breakpointStart = (double)kept_pos_sum / (double)remain;
         const double signalLen = (double)kept_len_sum / (double)remain;
+        // n ** 0.5 comes from a table of pow_n entries.  An allele at least that large reads entry 1 instead: it sets
+        // ST_POW_TABLE below, the host grows the table and reruns, and this call's records are discarded.
+        const int64_t n_pow = (uint32_t)n < E.lim.pow_n ? n : 1;
         // CIPOS / CILEN: np.std over the whole allele (:191-194); two lanes work concurrently
 #if defined(__CUDA_ARCH__)
         if (Team::SIZE == 32) {  // warp team: 16 lanes share the two reductions (n <= 128 here)
             auto g0 = [&](int i) { return (int64_t)D_pos[V3[st + i]]; };
             auto g1 = [&](int i) { return (int64_t)D_len[V3[st + i]]; };
             const double sd = warp_np_std2(g0, g1, n, sp, sl);
-            if (t == 0 || t == 8) red[t >> 3] = cal_cipos(sd, n, E.pow_half);
+            if (t == 0 || t == 8) red[t >> 3] = cal_cipos(sd, n_pow, E.pow_half);
         } else
 #endif
         if (Team::SIZE > 1) {
             if (t < 2) {  // lanes 0 / 1 run the SAME instruction stream on pos / len
                 const int32_t* src = t == 0 ? D_pos : D_len;
                 auto gv = [&](int64_t i) { return (int64_t)src[V3[st + i]]; };
-                red[t] = cal_cipos(np_std(gv, n, t == 0 ? sp : sl), n, E.pow_half);
+                red[t] = cal_cipos(np_std(gv, n, t == 0 ? sp : sl), n_pow, E.pow_half);
             }
         } else {
             auto gp = [&](int64_t i) { return (int64_t)D_pos[V3[st + i]]; };
-            red[0] = cal_cipos(np_std(gp, n, sp), n, E.pow_half);
+            red[0] = cal_cipos(np_std(gp, n, sp), n_pow, E.pow_half);
             auto gl = [&](int64_t i) { return (int64_t)D_len[V3[st + i]]; };
-            red[1] = cal_cipos(np_std(gl, n, sl), n, E.pow_half);
+            red[1] = cal_cipos(np_std(gl, n, sl), n_pow, E.pow_half);
         }
         tm.sync();
         const int32_t cipos = (int32_t)red[0], cilen = (int32_t)red[1];
