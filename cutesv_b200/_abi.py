@@ -14,6 +14,7 @@ TYPE_IDS = {n: i for i, n in enumerate(TYPE_NAMES)}
 CSV_OK, CSV_E_INVALID, CSV_E_CUDA, CSV_E_CAPACITY, CSV_E_NODEVICE, CSV_E_INPUT, CSV_E_STATE = (
     0, -1, -2, -3, -4, -5, -6)
 CSV_F_NO_READS, CSV_F_GT_HOST = 1, 2
+CSV_SORT_READS = 5   # csv_sort_sigs / csv_fetch_records: the reads table instead of one SV type
 
 STAGES = ("h2d", "keys", "sort", "segment", "cluster", "order", "genotype", "d2h", "extract")
 CSV_ST_COUNT = len(STAGES)

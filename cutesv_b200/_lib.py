@@ -54,6 +54,9 @@ _SIGNATURES = {
     "csv_swap_ins_rows": (C.c_int, [_VP, _I64P, C.c_int64]),
     "csv_fetch_sigs_range": (C.c_int, [_VP, C.c_int, C.c_int64, C.c_int64, _I32P, _I32P, _I32P, _I32P, _I32P, _I32P, _I32P]),
     "csv_fetch_pieces_range": (C.c_int, [_VP, C.c_int64, C.c_int64, _I32P]),
+    "csv_extract_records": (C.c_int, [_VP, C.c_int]),
+    "csv_fetch_records": (C.c_int, [_VP, C.c_int, C.c_int64, C.c_int64, _I32P]),
+    "csv_sort_sigs": (C.c_int, [_VP, C.c_int, _I64P, C.c_int64, _I64P, _I64P, C.POINTER(C.c_uint8)]),
     "csv_fetch_sigs": (C.c_int, [_VP, C.c_int, C.c_int64, _I32P, _I32P, _I32P, _I32P, _I32P, _I32P, _I32P]),
     "csv_fetch_pieces": (C.c_int, [_VP, C.c_int64, _I32P, _I64P]),
     "csv_fetch_read_rows": (C.c_int, [_VP, C.c_int64, _I32P, _I32P, _I32P, _I32P, C.POINTER(C.c_uint8)]),

@@ -477,12 +477,8 @@ def _write_workdir(tmp, sigs, reads_cols, chrom_names, read_names, ins_seq, writ
                                [chrom_names[i] for i in r["chrom"].tolist()]))
     workdir.write_workdir(tmp, tuples)
     if write_old_sigs:  # legacy text dumps, cuteSV:766-816
-        fmt = {"DEL": lambda e: "%s\t%s\t%d\t%d\t%s\n" % (e[-2], e[-1], e[0], e[1], e[2]),
-               "INS": lambda e: "%s\t%s\t%d\t%d\t%s\t%s\n" % (e[-2], e[-1], e[0], e[1], e[2], e[3]),
-               "DUP": lambda e: "%s\t%s\t%d\t%d\t%s\n" % (e[-2], e[-1], e[0], e[1], e[2]),
-               "INV": lambda e: "%s\t%s\t%s\t%d\t%d\t%s\n" % (e[-2], e[-1], e[0], e[1], e[2], e[3]),
-               "TRA": lambda e: "%s\t%s\t%s\t%d\t%s\t%d\t%s\n" % (e[-2], e[-1], e[0], e[1], e[2], e[3], e[4])}
-        for t, f in fmt.items():
+        for t in workdir.TYPES:
+            f = workdir.SIGS_LINE[t]
             with open("%s/%s.sigs" % (tmp, t), "w") as fh:
                 for e in sorted(set(tuples[t]), key=workdir.sort_key(t)):
                     fh.write(f(e))

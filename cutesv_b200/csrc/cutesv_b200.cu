@@ -90,6 +90,9 @@ struct SmallWork {  // DUP / INV / TRA
 
 struct ExtractState {
     DBuf r[7], cigar_off, sa_off, cigar, s[7], piece_off, piece_cnt, pieces, counters;
+    DBuf rec[CSV_NTYPES + 1];        // record index of every extracted signature per type / reads row (last)
+    bool rec_on = false;             // csv_extract_records: store the record column (off: no allocation, no stores)
+    bool rec_valid = false;          // the device-resident rows are csv_extract* output with the column stored for all of them
     uint32_t* h_counters = nullptr;  // pinned
     uint32_t n_pieces = 0;
     uint32_t n_records = 0;          // alignment records of all packets of the accumulation (record index base of INS pieces)
@@ -99,6 +102,7 @@ struct ExtractState {
 };
 static void extract_release(ExtractState* x) {
     for (int k = 0; k < 7; k++) { x->r[k].release(); x->s[k].release(); }
+    for (int k = 0; k <= CSV_NTYPES; k++) x->rec[k].release();
     x->cigar_off.release(); x->sa_off.release(); x->cigar.release(); x->piece_off.release(); x->piece_cnt.release();
     x->pieces.release(); x->counters.release();
     if (x->h_counters) cudaFreeHost(x->h_counters);
@@ -126,6 +130,15 @@ struct GcWork {
         DBuf* all[] = {&win, &bin_base, &bin_start, &bin_fill, &bin_list, &iter, &prim, &cov_off, &ovl_off, &cov_fill, &ovl_fill, &cov_u, &ovl_u,
                        &lb, &words, &r_chrom, &r_start, &r_end, &r_id, &r_prim, &cov_raw, &ovl_raw, &cov_ded, &ovl_ded, &cov_flag, &ovl_flag,
                        &sup_off, &sup, &geno};
+        for (DBuf* b : all) b->release();
+    }
+};
+
+// scratch of csv_sort_sigs (sigsort_api.inl): separate from everything csv_cluster uses
+struct SsWork {
+    DBuf keys_a, keys_b, vals_a, vals_b, keep, tie, kchrom, order, off, hist, lb, words;
+    void release() {
+        DBuf* all[] = {&keys_a, &keys_b, &vals_a, &vals_b, &keep, &tie, &kchrom, &order, &off, &hist, &lb, &words};
         for (DBuf* b : all) b->release();
     }
 };
@@ -247,6 +260,7 @@ struct csv_ctx {
     bool prev_is_chain_kernel = false;  // the launch being enqueued directly follows a chain kernel on the same stream
     DBuf cal_in0, cal_in1, cal_out, aln_flag;   // csv_cal_gl / csv_upload_alignments scratch (no per-call cudaMalloc)
     GcWork gc;                                  // csv_overlap_cover / csv_call_gt
+    SsWork ss;                                  // csv_sort_sigs
     int64_t pad_cand = 0, pad_names = 0;
     int64_t* h_gather = nullptr;    // pinned: per-rank headers after the gather
     int64_t g_n_cand = 0, g_n_names = 0;
@@ -497,6 +511,7 @@ extern "C" int csv_destroy(csv_ctx* c) {
                    &c->cal_out, &c->aln_flag, &c->scan_carry, &c->win_rec, &c->rest_list, &c->emit_cursor};
     for (DBuf* b : all) b->release();
     c->gc.release();
+    c->ss.release();
     for (auto& g : c->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
     if (c->comm) comm_destroy(c);
     if (c->h_gather) cudaFreeHost(c->h_gather);
@@ -658,6 +673,7 @@ static int upload_sigs_impl(csv_ctx* c, int t, const csv_sig_cols* h, const int6
     s.n = h->n;
     s.has_c = h->c != nullptr;
     c->counts_valid = false;
+    c->ex.rec_valid = false;
     if (h->n == 0) return CSV_OK;
     if ((!contig_off && !h->chrom) || !h->a || !h->b || !h->read_id) return set_err(CSV_E_INVALID, "null column");
     if ((t == CSV_INS || t == CSV_INV || t == CSV_TRA) && !h->c) return set_err(CSV_E_INVALID, "column c is required for INS/INV/TRA");
@@ -687,6 +703,7 @@ static int upload_reads_impl(csv_ctx* c, const csv_reads_cols* h, const int64_t*
     CU(cudaSetDevice(c->device));
     c->n_reads = h->n;
     c->counts_valid = false;
+    c->ex.rec_valid = false;
     if (h->n == 0) return CSV_OK;
     if ((!contig_off && !h->chrom) || !h->start || !h->end || !h->read_id || !h->is_primary) return set_err(CSV_E_INVALID, "null column");
     const size_t bytes = (size_t)h->n * 4;
@@ -1612,3 +1629,4 @@ extern "C" int csv_sort_probe(csv_ctx* c, float* ms_total, int64_t* bytes_total,
 #include "extract_api.inl"
 #include "gather_api.inl"
 #include "genotype_api.inl"
+#include "sigsort_api.inl"

@@ -105,6 +105,7 @@ __global__ void __launch_bounds__(EX_THREADS, EX_MIN_CTAS) k_extract(ReadView R,
             if (k < O.cap_rows) {
                 O.rr_chrom[k] = chrom; O.rr_start[k] = ref_start; O.rr_end[k] = ref_end; O.rr_id[k] = rid;
                 O.rr_prim[k] = (flag == 0 || flag == 16) ? 1 : 0;
+                if (O.rr_rec) O.rr_rec[k] = rec_base + (int32_t)rec;
             } else atomicOr(O.status, ST_LIST_OVERFLOW);
         }
         if (qlen < P.min_read_len) continue;  // parse_read, cuteSV:607

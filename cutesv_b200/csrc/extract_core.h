@@ -53,13 +53,18 @@ struct ExtractOut {
     uint32_t cap_rows;
     uint32_t* status;       // ST_* bits (overflow)
     uint32_t* n_skipped;    // records whose split-read analysis was skipped (more than MAX_SEGS segments), may be null
+    // record index (rec_base + packet index) of every signature / reads row, may be null.  One thread emits all rows of a
+    // record, so inside one record and type the slot order is the emission order of parse_read (cuteSV:606-681)
+    int32_t* rec_col[CSV_NTYPES];
+    int32_t* rr_rec;
 };
 
-CSV_HD int64_t emit_sig(const ExtractOut& O, int t, int32_t chrom, int32_t a, int32_t b, int32_t rid, int32_t c) {
+CSV_HD int64_t emit_sig(const ExtractOut& O, int t, int32_t chrom, int32_t a, int32_t b, int32_t rid, int32_t c, int32_t rec) {
     const uint32_t k = atomic_add_u32(&O.n_sig[t], 1u);
     if (k >= O.cap_sig[t]) { atomic_or_u32(O.status, ST_CAND_OVERFLOW); return -1; }
     O.col[t][0][k] = chrom; O.col[t][1][k] = a; O.col[t][2][k] = b; O.col[t][3][k] = rid;
     if (O.col[t][4]) O.col[t][4][k] = c;
+    if (O.rec_col[t]) O.rec_col[t][k] = rec;
     return (int64_t)k;
 }
 // reserve n pieces; returns first index or -1
@@ -71,7 +76,7 @@ CSV_HD int64_t reserve_pieces(const ExtractOut& O, uint32_t n) {
 CSV_HD void emit_ins_single(const ExtractOut& O, int32_t chrom, int32_t pos2x, int32_t len, int32_t rid, int32_t rec, int64_t a,
                             int64_t b, int64_t L, int rc) {
     const int32_t sl = py_slice_len(a, b, L);
-    const int64_t k = emit_sig(O, CSV_INS, chrom, pos2x, len, rid, sl);
+    const int64_t k = emit_sig(O, CSV_INS, chrom, pos2x, len, rid, sl, rec);
     if (k < 0) return;
     const int64_t p = reserve_pieces(O, 1);
     if (p < 0) { O.ins_piece_off[k] = 0; O.ins_piece_cnt[k] = 0; return; }
@@ -100,7 +105,7 @@ struct ReadCtx {
 
 CSV_HD void flush_ins(const ExtractOut& O, const ReadCtx& R, MergeState& S, const InsPiece* open_pieces) {
     if (!S.ins_open) return;
-    const int64_t k = emit_sig(O, CSV_INS, R.chrom, 2 * S.ins_pos, S.ins_len, R.rid, S.ins_seqlen);
+    const int64_t k = emit_sig(O, CSV_INS, R.chrom, 2 * S.ins_pos, S.ins_len, R.rid, S.ins_seqlen, R.rec);
     if (k >= 0) {
         // More merged insertions than the open-piece buffer holds (the reference has no limit, cuteSV:537-540): position, length
         // and len(seq) of the signature are complete; its piece list becomes ONE marker piece (rc == 2, start = reference
@@ -118,7 +123,7 @@ CSV_HD void flush_ins(const ExtractOut& O, const ReadCtx& R, MergeState& S, cons
 }
 CSV_HD void flush_del(const ExtractOut& O, const ReadCtx& R, MergeState& S) {
     if (!S.del_open) return;
-    emit_sig(O, CSV_DEL, R.chrom, S.del_pos, S.del_len, R.rid, 0);
+    emit_sig(O, CSV_DEL, R.chrom, S.del_pos, S.del_len, R.rid, 0, R.rec);
     S.del_open = 0;
 }
 // one qualifying insertion op: ref pos, length, query slice [qa, qb)
@@ -166,20 +171,20 @@ CSV_HD void analysis_inv(const SplitCtx& C, const Seg& e1, const Seg& e2) {  // 
     const int32_t sv = C.P.min_size;
     if (e1.strand == 0) {
         if (e1.fe - e2.fe >= sv)
-            if ((double)e2.rs + 0.5 * (double)(e1.fe - e2.fe) >= (double)e1.re) emit_sig(*C.O, CSV_INV, e1.chr, e2.fe, e1.fe, C.R.rid, 0);
+            if ((double)e2.rs + 0.5 * (double)(e1.fe - e2.fe) >= (double)e1.re) emit_sig(*C.O, CSV_INV, e1.chr, e2.fe, e1.fe, C.R.rid, 0, C.R.rec);
         if (e2.fe - e1.fe >= sv)
-            if ((double)e2.rs + 0.5 * (double)(e2.fe - e1.fe) >= (double)e1.re) emit_sig(*C.O, CSV_INV, e1.chr, e1.fe, e2.fe, C.R.rid, 0);
+            if ((double)e2.rs + 0.5 * (double)(e2.fe - e1.fe) >= (double)e1.re) emit_sig(*C.O, CSV_INV, e1.chr, e1.fe, e2.fe, C.R.rid, 0, C.R.rec);
     } else {
         if (e2.fs - e1.fs >= sv)
-            if ((double)e2.rs + 0.5 * (double)(e2.fs - e1.fs) >= (double)e1.re) emit_sig(*C.O, CSV_INV, e1.chr, e1.fs, e2.fs, C.R.rid, 1);
+            if ((double)e2.rs + 0.5 * (double)(e2.fs - e1.fs) >= (double)e1.re) emit_sig(*C.O, CSV_INV, e1.chr, e1.fs, e2.fs, C.R.rid, 1, C.R.rec);
         if (e1.fs - e2.fs >= sv)
-            if ((double)e2.rs + 0.5 * (double)(e1.fs - e2.fs) >= (double)e1.re) emit_sig(*C.O, CSV_INV, e1.chr, e2.fs, e1.fs, C.R.rid, 1);
+            if ((double)e2.rs + 0.5 * (double)(e1.fs - e2.fs) >= (double)e1.re) emit_sig(*C.O, CSV_INV, e1.chr, e2.fs, e1.fs, C.R.rid, 1, C.R.rec);
     }
 }
 
 // TRA signature: (type, pos1, chr2, pos2) tagged with chr1; c = chr2*4 + type
 CSV_HD void emit_tra(const SplitCtx& C, int type, int32_t pos1, int32_t chr2, int32_t pos2, int32_t chr1) {
-    emit_sig(*C.O, CSV_TRA, chr1, pos1, pos2, C.R.rid, chr2 * 4 + type);
+    emit_sig(*C.O, CSV_TRA, chr1, pos1, pos2, C.R.rid, chr2 * 4 + type, C.R.rec);
 }
 CSV_HD void analysis_bnd(const SplitCtx& C, const Seg& e1, const Seg& e2) {  // cuteSV:97-188
     if (!(e2.rs - e1.re <= 100)) return;
@@ -218,7 +223,7 @@ CSV_HD void del_pair(const SplitCtx& C, const Seg& e1, const Seg& e2, bool gate)
     const int64_t delta = (int64_t)e2.fs - e2.rs + e1.re - e1.fe;
     if ((double)(e1.fe - e2.fs) < dmax((double)C.P.min_size, (double)delta / 5.0) && delta >= C.P.min_size)
         if ((double)(e2.rs - e1.re) <= dmax(100.0, (double)delta / 5.0) && size_ok(C, delta))
-            if (gate) emit_sig(*C.O, CSV_DEL, e2.chr, e1.fe, (int32_t)delta, C.R.rid, 0);
+            if (gate) emit_sig(*C.O, CSV_DEL, e2.chr, e1.fe, (int32_t)delta, C.R.rid, 0, C.R.rec);
 }
 
 // segs[0..n): in insertion order (primary first, then SA entries); sorted here by read_start (stable)
@@ -244,7 +249,7 @@ CSV_HD void analysis_split_read(const SplitCtx& C, Seg* sp, int n) {
                         const int64_t h = trunc_half((int64_t)e2.fs - e1.fe);
                         emit_ins_single(*C.O, e2.chr, e1.fe + e2.fs, e2.rs + e1.fe - e2.fs - e1.re, C.R.rid, C.R.rec, (int64_t)e1.re + h,
                                         (int64_t)e2.rs - h, RL, rc ^ C.R.base_rc);
-                    } else emit_sig(*C.O, CSV_DUP, e2.chr, e2.fs, e1.fe, C.R.rid, 0);
+                    } else emit_sig(*C.O, CSV_DUP, e2.chr, e2.fs, e1.fe, C.R.rid, 0, C.R.rec);
                 }
                 ins_pair(C, e1, e2, rc, true);
                 del_pair(C, e1, e2, true);
@@ -262,15 +267,15 @@ CSV_HD void analysis_split_read(const SplitCtx& C, Seg* sp, int n) {
                             const double half = 0.5 * (double)(e3.fs - e1.fe);
                             if ((double)e2.rs + half >= (double)e1.re && (double)e3.rs + half >= (double)e2.re)
                                 if (e2.fs >= e1.fe && e3.fs >= e2.fe) {
-                                    emit_sig(*C.O, CSV_INV, e1.chr, e1.fe, e2.fe, C.R.rid, 0);
-                                    emit_sig(*C.O, CSV_INV, e1.chr, e2.fs, e3.fs, C.R.rid, 1);
+                                    emit_sig(*C.O, CSV_INV, e1.chr, e1.fe, e2.fe, C.R.rid, 0, C.R.rec);
+                                    emit_sig(*C.O, CSV_INV, e1.chr, e2.fs, e3.fs, C.R.rid, 1, C.R.rec);
                                 }
                         } else {  // -+-
                             const double half = 0.5 * (double)(e1.fs - e3.fe);
                             if ((double)e1.re <= (double)e2.rs + half && (double)e3.rs + half >= (double)e2.re)
                                 if (e2.fs - e3.fe >= -50 && e1.fs - e2.fe >= -50) {
-                                    emit_sig(*C.O, CSV_INV, e1.chr, e3.fe, e2.fe, C.R.rid, 0);
-                                    emit_sig(*C.O, CSV_INV, e1.chr, e2.fs, e1.fs, C.R.rid, 1);
+                                    emit_sig(*C.O, CSV_INV, e1.chr, e3.fe, e2.fe, C.R.rid, 0, C.R.rec);
+                                    emit_sig(*C.O, CSV_INV, e1.chr, e2.fs, e1.fs, C.R.rid, 1, C.R.rec);
                                 }
                         }
                     }
@@ -284,9 +289,9 @@ CSV_HD void analysis_split_read(const SplitCtx& C, Seg* sp, int n) {
                         if (e1.strand == 1) {
                             e1 = seg_flip(sp[a + 2], RL); e2 = seg_flip(sp[a + 1], RL); e3 = seg_flip(sp[a], RL); rc = 1;
                         }
-                        if (e2.fe - e3.fs >= sv && e2.fs < e3.fe) emit_sig(*C.O, CSV_DUP, e2.chr, e3.fs, e2.fe, C.R.rid, 0);
+                        if (e2.fe - e3.fs >= sv && e2.fs < e3.fe) emit_sig(*C.O, CSV_DUP, e2.chr, e3.fs, e2.fe, C.R.rid, 0, C.R.rec);
                         if (a == 0)
-                            if (e1.fe - e2.fs >= sv) emit_sig(*C.O, CSV_DUP, e2.chr, e2.fs, e1.fe, C.R.rid, 0);
+                            if (e1.fe - e2.fs >= sv) emit_sig(*C.O, CSV_DUP, e2.chr, e2.fs, e1.fe, C.R.rid, 0, C.R.rec);
                         const bool gate = e3.fs >= e2.fe;
                         ins_pair(C, e1, e2, rc, gate);
                         del_pair(C, e1, e2, gate);
@@ -331,7 +336,7 @@ CSV_HD void analysis_split_read(const SplitCtx& C, Seg* sp, int n) {
                 emit_ins_single(*C.O, e2.chr, 2 * pos, (int32_t)d, C.R.rid, C.R.rec, (int64_t)e1.re + h, (int64_t)e2.rs - h, RL,
                                 rc ^ C.R.base_rc);
             }
-            if (dis_ref <= -(int64_t)sv) emit_sig(*C.O, CSV_DUP, e2.chr, e2.fs, e1.fe, C.R.rid, 0);
+            if (dis_ref <= -(int64_t)sv) emit_sig(*C.O, CSV_DUP, e2.chr, e2.fs, e1.fe, C.R.rid, 0, C.R.rec);
         }
     }
 }

@@ -81,6 +81,7 @@ class Engine(object):
             keep.append(rk)
             _lib.check(self.L.csv_upload_reads(self.h, C.byref(r)))
         self._keep = keep  # host buffers must outlive the async copies
+        self._dev_rows = [len((sigs.get(n) or {}).get("a", ())) for n in _abi.TYPE_NAMES] + [0 if reads is None else len(reads["start"])]
 
     def upload_alignments(self, aln):
         """ALL alignment records in BAM order (dict like the reads table, is_primary = flag in (0, 16)): enables the
@@ -141,6 +142,7 @@ class Engine(object):
         nc, nn = C.c_int64(0), C.c_int64(0)
         tail = (C.c_uint32(type_mask), cands.ctypes.data_as(C.c_void_p), genos.ctypes.data_as(C.c_void_p), C.c_int64(len(cands)),
                 _abi.ptr(names), C.c_int64(len(names)), C.byref(nc), C.byref(nn))
+        self._dev_rows = [int(arr[t].n) for t in range(_abi.CSV_NTYPES)] + [int(r.n)]
         if grouped:
             _lib.check(self.L.csv_cluster_host_grouped(self.h, arr, offs, C.byref(r),
                                                        None if r_off is None else r_off.ctypes.data_as(C.POINTER(C.c_int64)), *tail))
@@ -202,6 +204,41 @@ class Engine(object):
                                       out.ctypes.data_as(C.c_void_p)))
         del keep
         return out[:n]
+
+    def sort_sigs(self, svtype):
+        """Sort + adjacent de-duplication of process_process_sigs_type (cuteSV:750-857, 958-969) over the device-resident
+        columns of one type (name or id) or of the reads table ("reads").  Returns dict(order, contig_off, ins_tie): the input
+        rows kept, in the reference's order; the row range of every contig id inside `order` (n_contigs + 1 offsets); for INS
+        the flags of rows that tie with their predecessor up to the sequence (zeros for the other types)."""
+        t = _abi.CSV_SORT_READS if svtype == "reads" else (_abi.TYPE_IDS[svtype] if isinstance(svtype, str) else int(svtype))
+        off = np.zeros(self.n_contigs + 1, np.int64)
+        nk = C.c_int64(0)
+        # the device-resident row count bounds the kept rows: one call, no capacity retry
+        cap = self._dev_rows[t] if getattr(self, "_dev_rows", None) is not None else 0
+        while True:
+            order = np.zeros(max(cap, 1), np.int64)
+            tie = np.zeros(max(cap, 1), np.uint8)
+            rc = self.L.csv_sort_sigs(self.h, C.c_int(t), order.ctypes.data_as(C.POINTER(C.c_int64)), C.c_int64(cap), C.byref(nk),
+                                      off.ctypes.data_as(C.POINTER(C.c_int64)), tie.ctypes.data_as(C.POINTER(C.c_uint8)))
+            if rc != _abi.CSV_E_CAPACITY:
+                break
+            cap = nk.value
+        _lib.check(rc)
+        n = nk.value
+        return dict(order=order[:n], contig_off=off, ins_tie=tie[:n])
+
+    def set_extract_records(self, on):
+        """Store the record index of every row of the following extract() calls (csv_extract_records), for fetch_records."""
+        _lib.check(self.L.csv_extract_records(self.h, int(bool(on))))
+
+    def fetch_records(self, svtype, first=0, count=None):
+        """Record index of extracted rows [first, first + count) of one type or of the reads table ("reads") (csv_fetch_records)."""
+        t = _abi.CSV_SORT_READS if svtype == "reads" else (_abi.TYPE_IDS[svtype] if isinstance(svtype, str) else int(svtype))
+        if count is None:
+            count = (self._ex_rows if t == _abi.CSV_SORT_READS else self._ex_counts[t]) - first
+        out = np.zeros(max(count, 1), np.int32)
+        _lib.check(self.L.csv_fetch_records(self.h, C.c_int(t), C.c_int64(first), C.c_int64(count), _abi.ptr(out)))
+        return out[:count]
 
     def stage_ms(self):
         ms = (C.c_float * _abi.CSV_ST_COUNT)()
@@ -349,6 +386,7 @@ def _extract_method(self, packed, append=False):
     _lib.check(fn(self.h, C.byref(rc_), cig.ctypes.data_as(C.POINTER(C.c_uint32)), C.c_int64(len(cig)), C.byref(sa_), counts, C.byref(n_rows)))
     self._ex_counts = [int(x) for x in counts]
     self._ex_rows = int(n_rows.value)
+    self._dev_rows = self._ex_counts + [self._ex_rows]
     self._ex_appending = bool(append)
     npz = C.c_int64(0)
     _lib.check(self.L.csv_fetch_pieces(self.h, C.c_int64(0), None, C.byref(npz)))
@@ -369,6 +407,7 @@ def _extract_reset_method(self):
     self._ex_rows = 0
     self._ex_pieces = 0
     self._ex_appending = False
+    self._dev_rows = [0] * (_abi.CSV_NTYPES + 1)
 
 
 def _fetch_ins_pieces_method(self, first_sig, n_sig, first_piece, n_piece):

@@ -27,6 +27,15 @@ def sort_key(svtype):
     return lambda x: (x[-1])
 
 
+# one line of the legacy --write_old_sigs text dumps (cuteSV:766-816)
+SIGS_LINE = {"DEL": lambda e: "%s\t%s\t%d\t%d\t%s\n" % (e[-2], e[-1], e[0], e[1], e[2]),
+             "INS": lambda e: "%s\t%s\t%d\t%d\t%s\t%s\n" % (e[-2], e[-1], e[0], e[1], e[2], e[3]),
+             "DUP": lambda e: "%s\t%s\t%d\t%d\t%s\n" % (e[-2], e[-1], e[0], e[1], e[2]),
+             "INV": lambda e: "%s\t%s\t%s\t%d\t%d\t%s\n" % (e[-2], e[-1], e[0], e[1], e[2], e[3]),
+             "TRA": lambda e: "%s\t%s\t%s\t%d\t%s\t%d\t%s\n" % (e[-2], e[-1], e[0], e[1], e[2], e[3], e[4]),
+             "reads": lambda e: "%s\t%d\t%d\t%d\t%s\n" % (e[-1], e[0], e[1], e[2], e[3])}
+
+
 def write_type(path, svtype, tuples):
     """Write <path><svtype>.pickle in the reference layout; returns (index, reads_count)."""
     cand = sorted(tuples, key=sort_key(svtype))
@@ -86,14 +95,15 @@ def _ids(values, index):
     return np.fromiter(map(index.__getitem__, values), dtype=np.int32, count=len(values))
 
 
-def tuples_to_columns(svtype, tuples, chrom_id, name_id):
-    """Reference tuples -> int32 columns, column-wise (zip(*tuples) transposes at C speed; no per-tuple Python loop)."""
+def tuples_to_columns(svtype, tuples, chrom_id, name_id, fields=None):
+    """Reference tuples -> int32 columns, column-wise (zip(*tuples) transposes at C speed; no per-tuple Python loop).
+    fields: list(zip(*tuples)) when the caller already has it."""
     n = len(tuples)
     cols = dict(chrom=np.zeros(n, np.int32), a=np.zeros(n, np.int32), b=np.zeros(n, np.int32), read_id=np.zeros(n, np.int32),
                 c=np.zeros(n, np.int32) if svtype in ("INS", "INV", "TRA") else None)
     if n == 0:
         return cols
-    f = list(zip(*tuples))
+    f = fields if fields is not None else list(zip(*tuples))
     cols["chrom"] = _ids(f[-1], chrom_id)
     if svtype == "DEL" or svtype == "DUP":
         cols["a"] = np.asarray(f[0], dtype=np.float64).astype(np.int32)   # int(): truncation
@@ -117,12 +127,12 @@ def tuples_to_columns(svtype, tuples, chrom_id, name_id):
     return cols
 
 
-def reads_to_columns(rows, chrom_id, name_id):
+def reads_to_columns(rows, chrom_id, name_id, fields=None):
     n = len(rows)
     if n == 0:
         return dict(chrom=np.zeros(0, np.int32), start=np.zeros(0, np.int32), end=np.zeros(0, np.int32), read_id=np.zeros(0, np.int32),
                     is_primary=np.zeros(0, np.uint8))
-    f = list(zip(*rows))
+    f = fields if fields is not None else list(zip(*rows))
     return dict(chrom=_ids(f[4], chrom_id), start=np.asarray(f[0], dtype=np.int64).astype(np.int32),
                 end=np.asarray(f[1], dtype=np.int64).astype(np.int32), read_id=_ids(f[3], name_id),
                 is_primary=np.asarray(f[2], dtype=np.int64).astype(np.uint8))

@@ -262,6 +262,30 @@ int csv_overlap_cover(csv_ctx* ctx, const csv_window* windows, int64_t n_windows
 int csv_call_gt(csv_ctx* ctx, const csv_window* windows, int64_t n_cand, int32_t windows_per_cand, const csv_reads_cols* reads,
                 const int64_t* support_off, const int32_t* support_ids, csv_geno* out);
 
+/* ---- standalone signature rebuild: the sort + remove_duplicates_sorted of process_process_sigs_type (cuteSV:750-857,
+ * 958-969) over the device-resident columns of ONE type (svtype CSV_DEL..CSV_TRA) or of the reads table
+ * (svtype CSV_SORT_READS), i.e. whatever csv_upload_sigs / csv_upload_reads (grouped or not) or csv_extract* put there ----
+ *
+ * Sort key, stable on input order (names and contigs are ranks), and what counts as an adjacent duplicate:
+ *   DEL, DUP  chrom, a, b, read_id                        all four fields equal
+ *   INV       chrom, c (strand), a, b, read_id            all five equal
+ *   TRA       chrom, c>>2 (chr2), c&3 (type), a, b, read_id   all five equal
+ *   INS       chrom, a>>1 (int(pos)), b, read_id          none dropped (see ins_tie)
+ *   reads     chrom                                       none dropped
+ * order[k] (k < *n_kept) = input row of the k-th kept row; contig_off (n_contigs + 1 entries) = row range of every contig
+ * id inside order, which is what the reference's per-contig pickle index needs.  On CSV_E_CAPACITY (*n_kept > cap) nothing
+ * but *n_kept is written.
+ * INS: the reference's key ends with the sequence string (cuteSV:774), which the library never sees.  ins_tie[k] = 1 when
+ * kept row k ties with row k - 1 on (chrom, int(pos), len, read_id); the host orders every such group by sequence
+ * (stably) and drops the adjacent duplicates (equal a, b, read_id and sequence).  The groups need one read reporting two
+ * equal insertions at one position, so they are rare.  ins_tie may be NULL; for other types it is zero-filled.
+ * Key widths follow the data (contig count, coordinates, read count), so > 32 768 contigs and genome spans > 2^32 sort as
+ * they are.  Own scratch: neither the device-resident inputs nor anything csv_cluster / csv_fetch return change.
+ * Input errors (CSV_E_INPUT): a contig id outside the contig table, a negative field.  Blocks until the results are on
+ * the host. */
+enum { CSV_SORT_READS = 5 };
+int csv_sort_sigs(csv_ctx* ctx, int svtype, int64_t* order, int64_t cap, int64_t* n_kept, int64_t* contig_off, uint8_t* ins_tie);
+
 /* ---- signature extraction: parse_read / generate_combine_sigs / organize_split_signal /
  * analysis_split_read (cuteSV:50-681) over a packet of decoded alignment records ---- */
 
@@ -325,6 +349,17 @@ int csv_swap_ins_rows(csv_ctx* ctx, const int64_t* pairs, int64_t n_pairs);
 int csv_fetch_sigs_range(csv_ctx* ctx, int svtype, int64_t first, int64_t count, int32_t* chrom, int32_t* a, int32_t* b,
                          int32_t* read_id, int32_t* c, int32_t* piece_off, int32_t* piece_cnt);
 int csv_fetch_pieces_range(csv_ctx* ctx, int64_t first, int64_t count, int32_t* pieces4);
+/* on != 0: the following csv_extract* calls also store the record index of every row they emit, for csv_fetch_records
+ * (4 B per row; default off, so an extraction that never asks for it pays nothing). */
+int csv_extract_records(csv_ctx* ctx, int on);
+/* Record index (position of the alignment record in the packet, plus the records of earlier packets of an append
+ * accumulation) of device-resident rows [first, first + count) of one type, or of the reads table (svtype 5).  The kernel
+ * hands out row slots with atomics, so rows come in no particular record order; but one thread emits all rows of a
+ * record, so a stable sort of the rows by this column restores the reference's list order (records in input order,
+ * inside a record the order in which parse_read appends, cuteSV:606-681, 729-733).  CSV_E_STATE when the device-resident
+ * rows were not produced by csv_extract* calls made with csv_extract_records on (or an upload or csv_swap_ins_rows came
+ * since). */
+int csv_fetch_records(csv_ctx* ctx, int svtype, int64_t first, int64_t count, int32_t* rec);
 /* D2H of the extracted signature columns of one type (parity tests, .sigs dumps, host ALT
  * strings).  piece_off / piece_cnt (INS only, may be NULL): slice of the piece table. */
 int csv_fetch_sigs(csv_ctx* ctx, int svtype, int64_t cap, int32_t* chrom, int32_t* a, int32_t* b,

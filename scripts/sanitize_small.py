@@ -1,5 +1,5 @@
 """Small end-to-end run for compute-sanitizer (memcheck / racecheck / initcheck): adversarial cases,
-a pile-up (CTA-class clusters), extraction and the TRA genotyper."""
+a pile-up (CTA-class clusters), extraction, the TRA genotyper and the standalone signature sort."""
 import sys, os
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -46,4 +46,10 @@ e.remap_read_ids(np.arange(len(rn), dtype=np.int32))
 for _ in range(3):
     e.cluster_device(0x1F)
 n += len(e.fetch()[0])
+# standalone signature sort + de-duplication (csv_sort_sigs) over the extracted columns and the reads table, with their
+# record column (csv_extract_records / csv_fetch_records)
+e.set_extract_records(True); e.extract(pk); e.set_extract_records(False)
+for t in list(_abi.TYPE_NAMES) + ["reads"]:
+    e.fetch_records(t)
+    n += len(e.sort_sigs(t)["order"])
 print("sanitize run ok, candidates:", n)
