@@ -153,6 +153,88 @@ def make_reads_cols(reads):
     return s, tuple(keep) + (prim,)
 
 
+SIG_FIELDS = ("chrom", "a", "b", "read_id", "c")
+READS_FIELDS = ("chrom", "start", "end", "read_id", "is_primary")
+_TYPESTR = {"is_primary": "|u1", "contig_off": "<i8"}   # every other column is int32 ("<i4")
+_ITEMSIZE = {"<i4": 4, "|u1": 1, "<i8": 8}
+
+
+def is_device_array(x):
+    """True for objects that expose __cuda_array_interface__ (torch CUDA tensors, CuPy / Numba device arrays)."""
+    try:
+        return hasattr(x, "__cuda_array_interface__")
+    except Exception:   # e.g. torch raises for a CPU tensor
+        return False
+
+
+def _device_index(x):
+    """Device ordinal an array reports (torch: .device.index, CuPy: .device.id), or None."""
+    d = getattr(x, "device", None)
+    for attr in ("index", "id"):
+        v = getattr(d, attr, None)
+        if isinstance(v, int):
+            return v
+    return None
+
+
+def device_cols(cols, fields, device, grouped=False, n_contigs=None):
+    """Normalises the columns of ONE upload (a signature dict of SIG_FIELDS or a reads dict of READS_FIELDS) whose columns live in
+    GPU memory.  Needs no GPU: it reads __cuda_array_interface__ and the arrays' device attribute only.
+
+    Returns None when the dict is None / empty or holds host columns only (the numpy path).  Otherwise (struct, contig_off address
+    or None): the csv_sig_cols / csv_reads_cols of device addresses for csv_upload_*_device.  grouped=True: the dict holds
+    `contig_off` (int64, n_contigs + 1) instead of `chrom`.
+    Raises TypeError for a column of the wrong dtype (int32; uint8 is_primary; int64 contig_off), not 1-D or not contiguous,
+    ValueError when host and device columns are mixed, when a column is on another device than `device`, or when lengths disagree.
+    Whether the addresses really are device memory of `device` is checked again by the library."""
+    if cols is None:
+        return None
+    names = [f for f in fields if not (grouped and f == "chrom")] + (["contig_off"] if grouped else [])
+    present = {f: cols.get(f) for f in names if cols.get(f) is not None}
+    on_dev = {f: is_device_array(v) for f, v in present.items()}
+    if not any(on_dev.values()):
+        return None
+    if not all(on_dev.values()):
+        raise ValueError("columns of one upload must be all device or all host arrays: host %s, device %s"
+                         % (sorted(f for f, d in on_dev.items() if not d), sorted(f for f, d in on_dev.items() if d)))
+    ptrs, lens = {}, {}
+    for f, v in present.items():
+        cai = v.__cuda_array_interface__
+        want = _TYPESTR.get(f, "<i4")
+        if cai["typestr"] != want:
+            raise TypeError("column %s: dtype %s, expected %s" % (f, cai["typestr"], want))
+        shape = tuple(cai["shape"])
+        if len(shape) != 1:
+            raise TypeError("column %s: shape %s, expected one dimension" % (f, shape))
+        strides = cai.get("strides")
+        if strides is not None and shape[0] > 1 and tuple(strides) != (_ITEMSIZE[want],):
+            raise TypeError("column %s is not contiguous (strides %s)" % (f, tuple(strides)))
+        idx = _device_index(v)
+        if idx is not None and idx != device:
+            raise ValueError("column %s is on device %d, the engine on device %d" % (f, idx, device))
+        ptrs[f] = int(cai["data"][0]) if shape[0] else None
+        lens[f] = shape[0]
+    row_cols = {f: n for f, n in lens.items() if f != "contig_off"}
+    if len(set(row_cols.values())) > 1:
+        raise ValueError("column lengths disagree: %s" % row_cols)
+    n = next(iter(row_cols.values()), 0)
+    for f in ("chrom", "a", "b", "read_id") if fields == SIG_FIELDS else ("chrom", "start", "end", "read_id", "is_primary"):
+        if f in names and f not in present and n:
+            raise ValueError("column %s is missing" % f)
+    off = None
+    if grouped and n:
+        if "contig_off" not in present:
+            raise ValueError("grouped columns need contig_off")
+        if n_contigs is not None and lens["contig_off"] != n_contigs + 1:
+            raise ValueError("contig_off has %d entries, expected n_contigs + 1 = %d" % (lens["contig_off"], n_contigs + 1))
+        off = C.cast(C.c_void_p(ptrs["contig_off"]), _I64P)
+    if fields == SIG_FIELDS:
+        s = csv_sig_cols(n, *[C.cast(C.c_void_p(ptrs.get(f) if n else None), _I32P) for f in SIG_FIELDS])
+    else:
+        s = csv_reads_cols(n, *[C.cast(C.c_void_p(ptrs.get(f) if n else None), _U8P if f == "is_primary" else _I32P) for f in READS_FIELDS])
+    return s, off
+
+
 def default_params(**kw):
     """Reference defaults (cuteSV_Description.py:78-262; wiring cuteSV:1116-1189)."""
     p = csv_params()

@@ -32,6 +32,11 @@ _SIGNATURES = {
     "csv_upload_sigs_grouped": (C.c_int, [_VP, C.c_int, C.POINTER(_abi.csv_sig_cols), _I64P]),
     "csv_upload_reads_grouped": (C.c_int, [_VP, C.POINTER(_abi.csv_reads_cols), _I64P]),
     "csv_upload_alignments": (C.c_int, [_VP, C.POINTER(_abi.csv_reads_cols)]),
+    "csv_upload_sigs_device": (C.c_int, [_VP, C.c_int, C.POINTER(_abi.csv_sig_cols), _VP]),
+    "csv_upload_reads_device": (C.c_int, [_VP, C.POINTER(_abi.csv_reads_cols), _VP]),
+    "csv_upload_sigs_grouped_device": (C.c_int, [_VP, C.c_int, C.POINTER(_abi.csv_sig_cols), _I64P, _VP]),
+    "csv_upload_reads_grouped_device": (C.c_int, [_VP, C.POINTER(_abi.csv_reads_cols), _I64P, _VP]),
+    "csv_upload_alignments_device": (C.c_int, [_VP, C.POINTER(_abi.csv_reads_cols), _VP]),
     "csv_cluster": (C.c_int, [_VP, C.c_uint32]),
     "csv_result_counts": (C.c_int, [_VP, _I64P, _I64P]),
     "csv_fetch": (C.c_int, [_VP, _VP, _VP, C.c_int64, _I32P, C.c_int64]),

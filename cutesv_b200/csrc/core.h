@@ -58,7 +58,8 @@ struct CudaTeam {
 // status word bits written by kernels (csv_ctx reports them as CSV_E_INPUT / internal errors)
 enum : uint32_t {
     ST_BAD_CHROM = 1u, ST_BAD_POS = 2u, ST_NEG_FIELD = 4u, ST_POW_TABLE = 8u, ST_CAND_OVERFLOW = 16u,
-    ST_NAMES_OVERFLOW = 32u, ST_LIST_OVERFLOW = 64u, ST_INTERNAL = 128u, ST_UNSORTED = 256u, ST_BIG_RUN = 512u, ST_SKIPPED = 1024u
+    ST_NAMES_OVERFLOW = 32u, ST_LIST_OVERFLOW = 64u, ST_INTERNAL = 128u, ST_UNSORTED = 256u, ST_BIG_RUN = 512u, ST_SKIPPED = 1024u,
+    ST_BAD_GROUPS = 2048u   // contig_off of a grouped upload from device memory is not 0 .. n non-decreasing
 };
 
 // counters block in device memory (one per csv_cluster call)

@@ -155,6 +155,10 @@ struct csv_ctx {
     cudaStream_t copy_stream = nullptr;
     cudaEvent_t ev_up[CSV_NTYPES + 1] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};  // last: reads table
     bool up_pending[CSV_NTYPES + 1] = {false, false, false, false, false, false};
+    bool up_device[CSV_NTYPES + 1] = {false, false, false, false, false, false};    // the pending upload copies device memory
+    bool up_checked[CSV_NTYPES + 1] = {false, false, false, false, false, false};   // the slot's offsets were checked on the device
+    DBuf up_status;                  // one word per slot: k_check_contig_off's result, folded into the next csv_cluster's status
+    cudaEvent_t ev_prod = nullptr;   // device uploads: end of the caller's work on its producer stream
     cudaEvent_t ev_done = nullptr;   // end of the last csv_cluster on the compute stream
     bool done_pending = false;
     int n_sm = 132;
@@ -230,6 +234,7 @@ struct csv_ctx {
     struct GraphKey {
         uint32_t mask; int64_t n[CSV_NTYPES]; int64_t n_reads, n_aln; csv_params P; int lanes; uint64_t alloc_epoch; uint64_t cfg_epoch;
         bool small_chain[CSV_NTYPES];
+        bool up_checked[CSV_NTYPES + 1];   // the chain folds these slots' device-side offset checks into its status
     };
     struct GraphSlot { bool valid = false; GraphKey key; cudaGraphExec_t exec = nullptr; int64_t launches = 0; uint64_t used = 0; };
     static constexpr int N_GRAPHS = 4;
@@ -446,6 +451,7 @@ extern "C" int csv_create(int device, void* stream, csv_ctx** out) {
         cudaError_t e4 = cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking);
         for (int i = 0; i <= CSV_NTYPES && e4 == cudaSuccess; i++) e4 = cudaEventCreateWithFlags(&c->ev_up[i], cudaEventDisableTiming);
         if (e4 == cudaSuccess) e4 = cudaEventCreateWithFlags(&c->ev_done, cudaEventDisableTiming);
+        if (e4 == cudaSuccess) e4 = cudaEventCreateWithFlags(&c->ev_prod, cudaEventDisableTiming);
         if (e4 == cudaSuccess) e4 = cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming);
         if (e4 == cudaSuccess) e4 = cudaStreamCreateWithFlags(&c->aux_stream, cudaStreamNonBlocking);
         if (e4 == cudaSuccess) e4 = cudaEventCreateWithFlags(&c->ev_aux, cudaEventDisableTiming);
@@ -477,6 +483,7 @@ extern "C" int csv_create(int device, void* stream, csv_ctx** out) {
     if (rc != CSV_OK) { delete c; return rc; }
     CU(c->d_epoch.ensure(64, true));
     CU(c->emit_cursor.ensure(256, true));
+    CU(c->up_status.ensure((CSV_NTYPES + 1) * 4, true));
     // opt in to large dynamic shared memory for the cluster kernels
     const int smem_warp = (CL_THREADS / 32) * WARP_M * ARENA_PER_MAX + (CL_THREADS / 32) * 40 * 8;
     CU(cudaFuncSetAttribute(k_cluster_warp<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_warp));
@@ -508,7 +515,7 @@ extern "C" int csv_destroy(csv_ctx* c) {
                    &c->small.perm_a, &c->small.perm_b, &c->small.sel, &c->small.u_chrom, &c->small.u_a, &c->small.u_b,
                    &c->small.u_rid, &c->small.u_c, &c->boff, &c->rec_a, &c->rec_b, &c->recc_a, &c->recc_b, &c->d_epoch,
                    &c->d_len_eff, &c->g_send, &c->g_recv, &c->g_cand, &c->g_geno, &c->g_names, &c->g_scratch, &c->g_tab, &c->cal_in0, &c->cal_in1,
-                   &c->cal_out, &c->aln_flag, &c->scan_carry, &c->win_rec, &c->rest_list, &c->emit_cursor};
+                   &c->cal_out, &c->aln_flag, &c->scan_carry, &c->win_rec, &c->rest_list, &c->emit_cursor, &c->up_status};
     for (DBuf* b : all) b->release();
     c->gc.release();
     c->ss.release();
@@ -544,6 +551,7 @@ extern "C" int csv_destroy(csv_ctx* c) {
     if (c->copy_stream) { cudaStreamSynchronize(c->copy_stream); cudaStreamDestroy(c->copy_stream); }
     for (int i = 0; i <= CSV_NTYPES; i++) if (c->ev_up[i]) cudaEventDestroy(c->ev_up[i]);
     if (c->ev_done) cudaEventDestroy(c->ev_done);
+    if (c->ev_prod) cudaEventDestroy(c->ev_prod);
     if (c->own_stream) cudaStreamDestroy(c->stream);
     delete c;
     return CSV_OK;
@@ -636,12 +644,50 @@ extern "C" int csv_set_profiling(csv_ctx* c, int on) {
 // ------------------------------------------------------------------------------------------
 // uploads
 // ------------------------------------------------------------------------------------------
-// The copy stream must not overwrite inputs that kernels of the previous csv_cluster still read.
-static int upload_begin(csv_ctx* c) {
+// Where the columns of one upload live.  Host columns (csv_upload_*) are H2D copies; device columns (csv_upload_*_device) are
+// device-to-device copies ordered after the work the caller enqueued on its producer stream, and that stream in turn waits for the
+// copies, so the caller may overwrite or free its buffers in stream order as soon as the call returns.  Either way the ctx owns
+// its inputs: csv_remap_read_ids / csv_swap_ins_rows rewrite them and captured graphs hold their addresses.
+struct UpSrc {
+    bool device;
+    cudaStream_t producer;   // device: the caller's stream (0 = the legacy default stream)
+    cudaMemcpyKind kind() const { return device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice; }
+};
+static const UpSrc HOST_SRC = {false, nullptr};
+
+// Device calls: every non-null column must be device (or managed) memory of the ctx's device.
+static int check_dev_col(const csv_ctx* c, const void* p, const char* name) {
+    if (!p) return CSV_OK;
+    cudaPointerAttributes a;
+    cudaError_t e = cudaPointerGetAttributes(&a, p);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return set_err(CSV_E_INVALID, "column %s: not a CUDA pointer (%s)", name, cudaGetErrorString(e));
+    }
+    if (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged)
+        return set_err(CSV_E_INVALID, "column %s is not device memory (host pointers go to the calls without _device)", name);
+    if (a.device != c->device) return set_err(CSV_E_INVALID, "column %s is on device %d, the ctx on device %d", name, a.device, c->device);
+    return CSV_OK;
+}
+
+// The copy stream must not overwrite inputs that kernels of the previous csv_cluster still read, nor read device columns before
+// the caller's producer stream wrote them.
+static int upload_begin(csv_ctx* c, const UpSrc& src) {
     if (c->done_pending) {
         CU(cudaStreamWaitEvent(c->copy_stream, c->ev_done, 0));
         c->done_pending = false;
     }
+    if (src.device) {
+        CU(cudaEventRecord(c->ev_prod, src.producer));
+        CU(cudaStreamWaitEvent(c->copy_stream, c->ev_prod, 0));
+    }
+    return CSV_OK;
+}
+static int upload_end(csv_ctx* c, int slot, const UpSrc& src) {
+    CU(cudaEventRecord(c->ev_up[slot], c->copy_stream));
+    if (src.device) CU(cudaStreamWaitEvent(src.producer, c->ev_up[slot], 0));
+    c->up_pending[slot] = true;
+    c->up_device[slot] = src.device;
     return CSV_OK;
 }
 static int wait_upload(csv_ctx* c, int slot) {
@@ -652,20 +698,32 @@ static int wait_upload(csv_ctx* c, int slot) {
     return CSV_OK;
 }
 // Grouped uploads: rows grouped by contig id (ascending) + n_contigs+1 row offsets instead of the 4-byte contig
-// column; the column is rebuilt on the device behind the copies (k_expand_contigs on the copy stream).
-static int stage_group_offsets(csv_ctx* c, int slot, const int64_t* off, int64_t n, int32_t* chrom_dev) {
+// column; the column is rebuilt on the device behind the copies (k_expand_contigs on the copy stream).  Host offsets are checked
+// here; device offsets are checked on the device (reading them here would need a synchronisation), and a failure is reported by
+// the next csv_cluster as CSV_E_INPUT.
+static int stage_group_offsets(csv_ctx* c, int slot, const int64_t* off, int64_t n, int32_t* chrom_dev, const UpSrc& src) {
     if (c->n_contigs == 0) return set_err(CSV_E_STATE, "csv_set_contigs has not been called");
-    if (off[0] != 0 || off[c->n_contigs] != n) return set_err(CSV_E_INVALID, "contig_off must start at 0 and end at n");
-    for (int k = 0; k < c->n_contigs; k++)
-        if (off[k + 1] < off[k]) return set_err(CSV_E_INVALID, "contig_off must be non-decreasing");
+    if (!src.device) {
+        if (off[0] != 0 || off[c->n_contigs] != n) return set_err(CSV_E_INVALID, "contig_off must start at 0 and end at n");
+        for (int k = 0; k < c->n_contigs; k++)
+            if (off[k + 1] < off[k]) return set_err(CSV_E_INVALID, "contig_off must be non-decreasing");
+    }
     CU(c->d_goff[slot].ensure(((size_t)c->n_contigs + 1) * 8));
-    CU(cudaMemcpyAsync(c->d_goff[slot].p, off, ((size_t)c->n_contigs + 1) * 8, cudaMemcpyHostToDevice, c->copy_stream));
-    k_expand_contigs<<<grid_for(c, n, 256 * 4), 256, 0, c->copy_stream>>>(c->d_goff[slot].as<int64_t>(), c->n_contigs, n, chrom_dev);
+    CU(cudaMemcpyAsync(c->d_goff[slot].p, off, ((size_t)c->n_contigs + 1) * 8, src.kind(), c->copy_stream));
+    uint32_t* bad = nullptr;
+    if (src.device) {
+        bad = c->up_status.as<uint32_t>() + slot;
+        CU(cudaMemsetAsync(bad, 0, 4, c->copy_stream));
+        k_check_contig_off<<<grid_for(c, (int64_t)c->n_contigs + 1, 256), 256, 0, c->copy_stream>>>(c->d_goff[slot].as<int64_t>(), c->n_contigs, n, bad);
+        c->launches++;
+        c->up_checked[slot] = true;
+    }
+    k_expand_contigs<<<grid_for(c, n, 256 * 4), 256, 0, c->copy_stream>>>(c->d_goff[slot].as<int64_t>(), c->n_contigs, n, chrom_dev, bad);
     c->launches++;
     return CSV_OK;
 }
 
-static int upload_sigs_impl(csv_ctx* c, int t, const csv_sig_cols* h, const int64_t* contig_off) {
+static int upload_sigs_impl(csv_ctx* c, int t, const csv_sig_cols* h, const int64_t* contig_off, const UpSrc& src) {
     if (!c || t < 0 || t >= CSV_NTYPES || !h) return set_err(CSV_E_INVALID, "bad argument");
     if (h->n < 0 || h->n >= (1ll << 30)) return set_err(CSV_E_INVALID, "signature count %lld out of range", (long long)h->n);
     CU(cudaSetDevice(c->device));
@@ -674,61 +732,89 @@ static int upload_sigs_impl(csv_ctx* c, int t, const csv_sig_cols* h, const int6
     s.has_c = h->c != nullptr;
     c->counts_valid = false;
     c->ex.rec_valid = false;
+    c->up_checked[t] = false;
     if (h->n == 0) return CSV_OK;
     if ((!contig_off && !h->chrom) || !h->a || !h->b || !h->read_id) return set_err(CSV_E_INVALID, "null column");
     if ((t == CSV_INS || t == CSV_INV || t == CSV_TRA) && !h->c) return set_err(CSV_E_INVALID, "column c is required for INS/INV/TRA");
+    int rc;
+    if (src.device) {
+        const void* col[6] = {contig_off ? nullptr : h->chrom, h->a, h->b, h->read_id, h->c, contig_off};
+        static const char* const nm[6] = {"chrom", "a", "b", "read_id", "c", "contig_off"};
+        for (int k = 0; k < 6; k++) if ((rc = check_dev_col(c, col[k], nm[k]))) return rc;
+    }
     const size_t bytes = (size_t)h->n * 4;
-    int rc = upload_begin(c);
+    const cudaMemcpyKind kind = src.kind();
+    rc = upload_begin(c, src);
     if (rc) return rc;
     CU(s.chrom.ensure(bytes)); CU(s.a.ensure(bytes)); CU(s.b.ensure(bytes)); CU(s.rid.ensure(bytes));
-    if (contig_off) { rc = stage_group_offsets(c, t, contig_off, h->n, s.chrom.as<int32_t>()); if (rc) return rc; }
-    else CU(cudaMemcpyAsync(s.chrom.p, h->chrom, bytes, cudaMemcpyHostToDevice, c->copy_stream));
-    CU(cudaMemcpyAsync(s.a.p, h->a, bytes, cudaMemcpyHostToDevice, c->copy_stream));
-    CU(cudaMemcpyAsync(s.b.p, h->b, bytes, cudaMemcpyHostToDevice, c->copy_stream));
-    CU(cudaMemcpyAsync(s.rid.p, h->read_id, bytes, cudaMemcpyHostToDevice, c->copy_stream));
-    if (h->c) { CU(s.c.ensure(bytes)); CU(cudaMemcpyAsync(s.c.p, h->c, bytes, cudaMemcpyHostToDevice, c->copy_stream)); }
-    CU(cudaEventRecord(c->ev_up[t], c->copy_stream));
-    c->up_pending[t] = true;
-    return CSV_OK;
+    if (contig_off) { rc = stage_group_offsets(c, t, contig_off, h->n, s.chrom.as<int32_t>(), src); if (rc) return rc; }
+    else CU(cudaMemcpyAsync(s.chrom.p, h->chrom, bytes, kind, c->copy_stream));
+    CU(cudaMemcpyAsync(s.a.p, h->a, bytes, kind, c->copy_stream));
+    CU(cudaMemcpyAsync(s.b.p, h->b, bytes, kind, c->copy_stream));
+    CU(cudaMemcpyAsync(s.rid.p, h->read_id, bytes, kind, c->copy_stream));
+    if (h->c) { CU(s.c.ensure(bytes)); CU(cudaMemcpyAsync(s.c.p, h->c, bytes, kind, c->copy_stream)); }
+    return upload_end(c, t, src);
 }
-extern "C" int csv_upload_sigs(csv_ctx* c, int t, const csv_sig_cols* h) { return upload_sigs_impl(c, t, h, nullptr); }
+extern "C" int csv_upload_sigs(csv_ctx* c, int t, const csv_sig_cols* h) { return upload_sigs_impl(c, t, h, nullptr, HOST_SRC); }
 extern "C" int csv_upload_sigs_grouped(csv_ctx* c, int t, const csv_sig_cols* h, const int64_t* contig_off) {
     if (!contig_off) return set_err(CSV_E_INVALID, "null contig_off");
-    return upload_sigs_impl(c, t, h, contig_off);
+    return upload_sigs_impl(c, t, h, contig_off, HOST_SRC);
+}
+extern "C" int csv_upload_sigs_device(csv_ctx* c, int t, const csv_sig_cols* d, void* stream) {
+    return upload_sigs_impl(c, t, d, nullptr, UpSrc{true, (cudaStream_t)stream});
+}
+extern "C" int csv_upload_sigs_grouped_device(csv_ctx* c, int t, const csv_sig_cols* d, const int64_t* contig_off, void* stream) {
+    if (!contig_off) return set_err(CSV_E_INVALID, "null contig_off");
+    return upload_sigs_impl(c, t, d, contig_off, UpSrc{true, (cudaStream_t)stream});
 }
 
-static int upload_reads_impl(csv_ctx* c, const csv_reads_cols* h, const int64_t* contig_off) {
+static int upload_reads_impl(csv_ctx* c, const csv_reads_cols* h, const int64_t* contig_off, const UpSrc& src) {
     if (!c || !h) return set_err(CSV_E_INVALID, "bad argument");
     if (h->n < 0 || h->n >= (1ll << 31)) return set_err(CSV_E_INVALID, "read count out of range");
     CU(cudaSetDevice(c->device));
     c->n_reads = h->n;
     c->counts_valid = false;
     c->ex.rec_valid = false;
+    c->up_checked[CSV_NTYPES] = false;
     if (h->n == 0) return CSV_OK;
     if ((!contig_off && !h->chrom) || !h->start || !h->end || !h->read_id || !h->is_primary) return set_err(CSV_E_INVALID, "null column");
+    int rc;
+    if (src.device) {
+        const void* col[6] = {contig_off ? nullptr : h->chrom, h->start, h->end, h->read_id, h->is_primary, contig_off};
+        static const char* const nm[6] = {"chrom", "start", "end", "read_id", "is_primary", "contig_off"};
+        for (int k = 0; k < 6; k++) if ((rc = check_dev_col(c, col[k], nm[k]))) return rc;
+    }
     const size_t bytes = (size_t)h->n * 4;
-    int rc = upload_begin(c);
+    const cudaMemcpyKind kind = src.kind();
+    rc = upload_begin(c, src);
     if (rc) return rc;
     CU(c->r_chrom.ensure(bytes)); CU(c->r_start.ensure(bytes)); CU(c->r_end.ensure(bytes)); CU(c->r_id.ensure(bytes));
     CU(c->r_prim.ensure((size_t)h->n));
-    if (contig_off) { rc = stage_group_offsets(c, CSV_NTYPES, contig_off, h->n, c->r_chrom.as<int32_t>()); if (rc) return rc; }
-    else CU(cudaMemcpyAsync(c->r_chrom.p, h->chrom, bytes, cudaMemcpyHostToDevice, c->copy_stream));
-    CU(cudaMemcpyAsync(c->r_start.p, h->start, bytes, cudaMemcpyHostToDevice, c->copy_stream));
-    CU(cudaMemcpyAsync(c->r_end.p, h->end, bytes, cudaMemcpyHostToDevice, c->copy_stream));
-    CU(cudaMemcpyAsync(c->r_id.p, h->read_id, bytes, cudaMemcpyHostToDevice, c->copy_stream));
-    CU(cudaMemcpyAsync(c->r_prim.p, h->is_primary, (size_t)h->n, cudaMemcpyHostToDevice, c->copy_stream));
-    CU(cudaEventRecord(c->ev_up[CSV_NTYPES], c->copy_stream));
-    c->up_pending[CSV_NTYPES] = true;
-    return CSV_OK;
+    if (contig_off) { rc = stage_group_offsets(c, CSV_NTYPES, contig_off, h->n, c->r_chrom.as<int32_t>(), src); if (rc) return rc; }
+    else CU(cudaMemcpyAsync(c->r_chrom.p, h->chrom, bytes, kind, c->copy_stream));
+    CU(cudaMemcpyAsync(c->r_start.p, h->start, bytes, kind, c->copy_stream));
+    CU(cudaMemcpyAsync(c->r_end.p, h->end, bytes, kind, c->copy_stream));
+    CU(cudaMemcpyAsync(c->r_id.p, h->read_id, bytes, kind, c->copy_stream));
+    CU(cudaMemcpyAsync(c->r_prim.p, h->is_primary, (size_t)h->n, kind, c->copy_stream));
+    return upload_end(c, CSV_NTYPES, src);
 }
 
-extern "C" int csv_upload_reads(csv_ctx* c, const csv_reads_cols* h) { return upload_reads_impl(c, h, nullptr); }
+extern "C" int csv_upload_reads(csv_ctx* c, const csv_reads_cols* h) { return upload_reads_impl(c, h, nullptr, HOST_SRC); }
 extern "C" int csv_upload_reads_grouped(csv_ctx* c, const csv_reads_cols* h, const int64_t* contig_off) {
     if (!contig_off) return set_err(CSV_E_INVALID, "null contig_off");
-    return upload_reads_impl(c, h, contig_off);
+    return upload_reads_impl(c, h, contig_off, HOST_SRC);
+}
+extern "C" int csv_upload_reads_device(csv_ctx* c, const csv_reads_cols* d, void* stream) {
+    return upload_reads_impl(c, d, nullptr, UpSrc{true, (cudaStream_t)stream});
+}
+extern "C" int csv_upload_reads_grouped_device(csv_ctx* c, const csv_reads_cols* d, const int64_t* contig_off, void* stream) {
+    if (!contig_off) return set_err(CSV_E_INVALID, "null contig_off");
+    return upload_reads_impl(c, d, contig_off, UpSrc{true, (cudaStream_t)stream});
 }
 
-extern "C" int csv_upload_alignments(csv_ctx* c, const csv_reads_cols* h) {
+// The alignment table is copied on the ctx stream and its order is checked before the call returns (one synchronisation, for host
+// and device columns alike), so a device source's buffers are free again on return.
+static int upload_alignments_impl(csv_ctx* c, const csv_reads_cols* h, const UpSrc& src) {
     if (!c || !h) return set_err(CSV_E_INVALID, "bad argument");
     if (c->n_contigs == 0) return set_err(CSV_E_STATE, "csv_set_contigs has not been called");
     if (h->n < 0 || h->n >= (1ll << 31)) return set_err(CSV_E_INVALID, "alignment count out of range");
@@ -737,16 +823,26 @@ extern "C" int csv_upload_alignments(csv_ctx* c, const csv_reads_cols* h) {
     c->counts_valid = false;
     if (h->n == 0) return CSV_OK;
     if (!h->chrom || !h->start || !h->end || !h->read_id || !h->is_primary) return set_err(CSV_E_INVALID, "null column");
+    if (src.device) {
+        const void* col[5] = {h->chrom, h->start, h->end, h->read_id, h->is_primary};
+        static const char* const nm[5] = {"chrom", "start", "end", "read_id", "is_primary"};
+        for (int k = 0; k < 5; k++) { int rc = check_dev_col(c, col[k], nm[k]); if (rc) return rc; }
+    }
     const size_t bytes = (size_t)h->n * 4;
+    const cudaMemcpyKind kind = src.kind();
     CU(c->a_chrom.ensure(bytes)); CU(c->a_start.ensure(bytes)); CU(c->a_end.ensure(bytes)); CU(c->a_id.ensure(bytes));
     CU(c->a_prim.ensure((size_t)h->n));
     CU(c->a_off.ensure(((size_t)c->n_contigs + 2) * 4)); CU(c->a_span.ensure(((size_t)c->n_contigs + 2) * 4));
     CU(c->counters.ensure(sizeof(Counters)));
-    CU(cudaMemcpyAsync(c->a_chrom.p, h->chrom, bytes, cudaMemcpyHostToDevice, c->stream));
-    CU(cudaMemcpyAsync(c->a_start.p, h->start, bytes, cudaMemcpyHostToDevice, c->stream));
-    CU(cudaMemcpyAsync(c->a_end.p, h->end, bytes, cudaMemcpyHostToDevice, c->stream));
-    CU(cudaMemcpyAsync(c->a_id.p, h->read_id, bytes, cudaMemcpyHostToDevice, c->stream));
-    CU(cudaMemcpyAsync(c->a_prim.p, h->is_primary, (size_t)h->n, cudaMemcpyHostToDevice, c->stream));
+    if (src.device) {
+        CU(cudaEventRecord(c->ev_prod, src.producer));
+        CU(cudaStreamWaitEvent(c->stream, c->ev_prod, 0));
+    }
+    CU(cudaMemcpyAsync(c->a_chrom.p, h->chrom, bytes, kind, c->stream));
+    CU(cudaMemcpyAsync(c->a_start.p, h->start, bytes, kind, c->stream));
+    CU(cudaMemcpyAsync(c->a_end.p, h->end, bytes, kind, c->stream));
+    CU(cudaMemcpyAsync(c->a_id.p, h->read_id, bytes, kind, c->stream));
+    CU(cudaMemcpyAsync(c->a_prim.p, h->is_primary, (size_t)h->n, kind, c->stream));
     // contig index + sortedness check (BAM order is a precondition of the early-exit scan)
     CU(c->aln_flag.ensure(64));
     uint32_t* flag = c->aln_flag.as<uint32_t>();
@@ -763,6 +859,10 @@ extern "C" int csv_upload_alignments(csv_ctx* c, const csv_reads_cols* h) {
         return set_err(CSV_E_INPUT, "alignment table: %s", (hflag & ST_UNSORTED) ? "not coordinate-sorted (BAM order required)" : "contig id out of range");
     }
     return CSV_OK;
+}
+extern "C" int csv_upload_alignments(csv_ctx* c, const csv_reads_cols* h) { return upload_alignments_impl(c, h, HOST_SRC); }
+extern "C" int csv_upload_alignments_device(csv_ctx* c, const csv_reads_cols* d, void* stream) {
+    return upload_alignments_impl(c, d, UpSrc{true, (cudaStream_t)stream});
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1284,6 +1384,7 @@ static int enqueue_cluster(csv_ctx* c, uint32_t type_mask) {
             lane_swap(c, *L);   // c->stream and the scratch buffers are the lane's until swapped back
         }
         rc = wait_upload(c, t);
+        if (!rc && c->up_checked[t]) LAUNCH(c, k_fold_status, 1, 32, 0, c->up_status.as<uint32_t>() + t, &ctr->status);
         if (!rc) rc = (t == CSV_DEL || t == CSV_INS) ? run_indel(c, t, kslot_base) : run_other(c, t, kslot_base);
         if (L) lane_swap(c, *L);
         if (rc) {   // the ctx stream must not run ahead of work already forked
@@ -1342,6 +1443,8 @@ static int enqueue_cluster(csv_ctx* c, uint32_t type_mask) {
     // ---- genotype ----
     rc = wait_upload(c, CSV_NTYPES);
     if (rc) return rc;
+    if (c->up_checked[CSV_NTYPES] && c->n_reads > 0)
+        LAUNCH(c, k_fold_status, 1, 32, 0, c->up_status.as<uint32_t>() + CSV_NTYPES, &ctr->status);
     stage_begin(c, CSV_ST_GENOTYPE);
     {
         if (c->P.genotype) {
@@ -1404,15 +1507,21 @@ extern "C" int csv_cluster(csv_ctx* c, uint32_t type_mask) {
     }
     // A call whose inputs are already resident (no upload in flight) and that is not being profiled replays a
     // captured CUDA graph: first sighting of a key runs eagerly (buffers get their sizes), the second captures,
-    // later ones replay -- ~40 launches on 6 streams become one cudaGraphLaunch.
+    // later ones replay -- ~40 launches on 6 streams become one cudaGraphLaunch.  Device-to-device uploads are waited for here,
+    // before the chain (they take a fraction of the chain's time), so that a call on fresh device inputs still replays; host
+    // uploads keep their per-type waits, which let the H2D copies of later types overlap the kernels of earlier ones.
     bool pending = false;
-    for (int t = 0; t <= CSV_NTYPES; t++) pending |= c->up_pending[t];
+    for (int t = 0; t <= CSV_NTYPES; t++) {
+        if (c->up_pending[t] && c->up_device[t]) { rc = wait_upload(c, t); if (rc) return rc; }
+        pending |= c->up_pending[t];
+    }
     bool done = false;
     if (c->graphs_enabled && !c->profiling && !pending) {
         csv_ctx::GraphKey key;
         memset(&key, 0, sizeof(key));
         key.mask = type_mask;
         for (int t = 0; t < CSV_NTYPES; t++) { key.n[t] = c->sig[t].n; key.small_chain[t] = c->small_chain[t]; }
+        for (int t = 0; t <= CSV_NTYPES; t++) key.up_checked[t] = c->up_checked[t];
         key.n_reads = c->n_reads; key.n_aln = c->n_aln; key.P = c->P; key.lanes = c->lanes_enabled ? 1 : 0;
         key.alloc_epoch = g_alloc_epoch.load(); key.cfg_epoch = c->cfg_epoch;
         csv_ctx::GraphSlot* hit = nullptr;
@@ -1470,9 +1579,10 @@ static int finish(csv_ctx* c) {
     CU(cudaMemcpyAsync(c->h_counters, c->counters.p, sizeof(Counters), cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     const uint32_t st = c->h_counters->status;
-    if (st & (ST_BAD_CHROM | ST_BAD_POS | ST_NEG_FIELD))
-        return set_err(CSV_E_INPUT, "input validation failed on the device: %s%s%s", (st & ST_BAD_CHROM) ? "[contig id out of range] " : "",
-                       (st & ST_BAD_POS) ? "[position outside its contig] " : "", (st & ST_NEG_FIELD) ? "[negative field] " : "");
+    if (st & (ST_BAD_CHROM | ST_BAD_POS | ST_NEG_FIELD | ST_BAD_GROUPS))
+        return set_err(CSV_E_INPUT, "input validation failed on the device: %s%s%s%s", (st & ST_BAD_CHROM) ? "[contig id out of range] " : "",
+                       (st & ST_BAD_POS) ? "[position outside its contig] " : "", (st & ST_NEG_FIELD) ? "[negative field] " : "",
+                       (st & ST_BAD_GROUPS) ? "[contig_off of a grouped device upload is not 0 .. n, non-decreasing] " : "");
     if (st & ST_POW_TABLE) {
         // an allele with more supporting reads than the n**0.5 table: grow the table and rerun
         uint32_t need = c->h_counters->max_support + 1;
@@ -1542,12 +1652,12 @@ static int cluster_host_impl(csv_ctx* c, const csv_sig_cols sigs[CSV_NTYPES], co
     for (int t = 0; t < CSV_NTYPES; t++) {
         if (!(type_mask >> t & 1)) continue;
         if (grouped && sigs[t].n > 0 && (!sig_off || !sig_off[t])) return set_err(CSV_E_INVALID, "null contig_off");
-        rc = upload_sigs_impl(c, t, &sigs[t], grouped && sigs[t].n > 0 ? sig_off[t] : nullptr);
+        rc = upload_sigs_impl(c, t, &sigs[t], grouped && sigs[t].n > 0 ? sig_off[t] : nullptr, HOST_SRC);
         if (rc) return rc;
     }
     if (reads) {
         if (grouped && reads->n > 0 && !reads_off) return set_err(CSV_E_INVALID, "null contig_off");
-        rc = upload_reads_impl(c, reads, grouped && reads->n > 0 ? reads_off : nullptr);
+        rc = upload_reads_impl(c, reads, grouped && reads->n > 0 ? reads_off : nullptr, HOST_SRC);
         if (rc) return rc;
     }
     rc = csv_cluster(c, type_mask);

@@ -237,8 +237,31 @@ struct ContigTab {
 static constexpr int BKT_SHIFT = 8;   // 256 bp buckets
 static constexpr int BKT_PAD = 64;   // >= largest neighbourhood radius in buckets
 
-// grouped uploads: chrom[i] = the contig k with off[k] <= i < off[k+1] (four consecutive rows per thread)
-__global__ void __launch_bounds__(256) k_expand_contigs(const int64_t* __restrict__ off, int n_contigs, int64_t n, int32_t* __restrict__ chrom) {
+// grouped uploads from device memory: the offsets were never seen by the host, so they are checked here (off[0] == 0,
+// off[n_contigs] == n, non-decreasing) before k_expand_contigs trusts them; reads only the n_contigs + 1 offsets
+__global__ void __launch_bounds__(256) k_check_contig_off(const int64_t* __restrict__ off, int n_contigs, int64_t n, uint32_t* bad) {
+    bool ok = true;
+    for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k <= n_contigs; k += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t o = off[k];
+        if (k == 0 && o != 0) ok = false;
+        if (k == n_contigs && o != n) ok = false;
+        if (k < n_contigs && off[k + 1] < o) ok = false;
+    }
+    if (!ok) atomicOr(bad, ST_BAD_GROUPS);
+}
+// csv_cluster: an upload's device-side check result joins the call's status word (the upload ran before the counters were reset)
+__global__ void k_fold_status(const uint32_t* __restrict__ src, uint32_t* dst) {
+    if (threadIdx.x == 0 && *src) atomicOr(dst, *src);
+}
+
+// grouped uploads: chrom[i] = the contig k with off[k] <= i < off[k+1] (four consecutive rows per thread).
+// bad != nullptr: the result of k_check_contig_off; failed offsets give contig 0 to every row instead (never read out of range)
+__global__ void __launch_bounds__(256) k_expand_contigs(const int64_t* __restrict__ off, int n_contigs, int64_t n, int32_t* __restrict__ chrom,
+                                                        const uint32_t* __restrict__ bad) {
+    if (bad && *bad) {
+        for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) chrom[i] = 0;
+        return;
+    }
     for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v * 4 < n; v += (int64_t)gridDim.x * blockDim.x) {
         const int64_t i0 = v * 4;
         int lo = 0, hi = n_contigs;   // last k with off[k] <= i0

@@ -53,12 +53,48 @@ class Engine(object):
 
     # -- device-resident path (bench `value`): upload once, cluster many times --
 
-    def upload(self, sigs, reads, grouped=False):
+    def _producer_stream(self, stream, groups):
+        """cudaStream_t of device uploads: `stream` (a handle or a torch.cuda.Stream); else torch's current stream on the engine's
+        device when a column is a torch tensor; else 0 (the legacy default stream)."""
+        if stream is not None:
+            return int(getattr(stream, "cuda_stream", stream))
+        for cols in groups:
+            for v in (cols or {}).values():
+                if _abi.is_device_array(v) and type(v).__module__.startswith("torch"):
+                    import torch
+                    return int(torch.cuda.current_stream(self.device).cuda_stream)
+        return 0
+
+    def _upload_device(self, t, d, stream):
+        """csv_upload_*_device of one normalised column set (_abi.device_cols); t = SV type id, or None for the reads table."""
+        s, off = d
+        st = C.c_void_p(stream or None)
+        if t is None:
+            if off is not None:
+                _lib.check(self.L.csv_upload_reads_grouped_device(self.h, C.byref(s), off, st))
+            else:
+                _lib.check(self.L.csv_upload_reads_device(self.h, C.byref(s), st))
+        elif off is not None:
+            _lib.check(self.L.csv_upload_sigs_grouped_device(self.h, t, C.byref(s), off, st))
+        else:
+            _lib.check(self.L.csv_upload_sigs_device(self.h, t, C.byref(s), st))
+
+    def upload(self, sigs, reads, grouped=False, stream=None):
         """Asynchronous H2D of the inputs of cluster_device().  grouped=True: dicts from _abi.group_by_contig (rows grouped by
-        contig + `contig_off` instead of the contig column; csv_upload_*_grouped)."""
+        contig + `contig_off` instead of the contig column; csv_upload_*_grouped).
+        Column dicts whose arrays expose __cuda_array_interface__ (torch CUDA tensors) are copied device-to-device instead
+        (csv_upload_*_device), in the order of `stream` (see _producer_stream): the copies follow the work already enqueued on it,
+        and work enqueued on it after this call (overwriting or freeing the tensors) follows the copies.  One dict is all device
+        or all host; device signatures with host reads (or the reverse) are fine."""
+        n_contigs = getattr(self, "n_contigs", None)
+        dev = {name: _abi.device_cols(sigs.get(name), _abi.SIG_FIELDS, self.device, grouped, n_contigs) for name in _abi.TYPE_NAMES}
+        dev_r = _abi.device_cols(reads, _abi.READS_FIELDS, self.device, grouped, n_contigs)
+        st = self._producer_stream(stream, list(sigs.values()) + [reads]) if dev_r or any(dev.values()) else 0
         keep = []
         for t, name in enumerate(_abi.TYPE_NAMES):
-            if grouped:
+            if dev[name] is not None:
+                self._upload_device(t, dev[name], st)
+            elif grouped:
                 s, off, k = _abi.make_sig_cols_grouped(sigs.get(name))
                 keep.append((k, off))
                 if off is not None:
@@ -69,7 +105,9 @@ class Engine(object):
                 s, k = _abi.make_sig_cols(sigs.get(name))
                 keep.append(k)
                 _lib.check(self.L.csv_upload_sigs(self.h, t, C.byref(s)))
-        if grouped:
+        if dev_r is not None:
+            self._upload_device(None, dev_r, st)
+        elif grouped:
             r, r_off, rk = _abi.make_reads_cols_grouped(reads)
             keep.append((rk, r_off))
             if r_off is not None:
@@ -83,9 +121,16 @@ class Engine(object):
         self._keep = keep  # host buffers must outlive the async copies
         self._dev_rows = [len((sigs.get(n) or {}).get("a", ())) for n in _abi.TYPE_NAMES] + [0 if reads is None else len(reads["start"])]
 
-    def upload_alignments(self, aln):
+    def upload_alignments(self, aln, stream=None):
         """ALL alignment records in BAM order (dict like the reads table, is_primary = flag in (0, 16)): enables the
-        device TRA genotyper (call_gt, resolveTRA.py:260-309).  None / empty clears the table."""
+        device TRA genotyper (call_gt, resolveTRA.py:260-309).  None / empty clears the table.  Device columns (torch CUDA
+        tensors) go through csv_upload_alignments_device in the order of `stream`, as in upload()."""
+        d = _abi.device_cols(aln, _abi.READS_FIELDS, self.device)
+        if d is not None:
+            st = self._producer_stream(stream, [aln])
+            _lib.check(self.L.csv_upload_alignments_device(self.h, C.byref(d[0]), C.c_void_p(st or None)))
+            self._keep_aln = ()
+            return
         r, keep = _abi.make_reads_cols(aln)
         _lib.check(self.L.csv_upload_alignments(self.h, C.byref(r)))
         self._keep_aln = keep
@@ -93,26 +138,47 @@ class Engine(object):
     def cluster_device(self, type_mask=0x1F):
         _lib.check(self.L.csv_cluster(self.h, C.c_uint32(type_mask)))
 
+    def result_tensors(self):
+        """Zero-copy torch views of the last cluster call's results on the engine's device (csv_result_device_ptrs):
+        (cands [n, 16] int32 = csv_cand, genos [n, 10] int32 = csv_geno (qual is the float64 in words 8-9), names int32).
+        Blocks until the results are ready.  The views alias the engine's own buffers: they are valid until the next upload,
+        cluster call or close() on this engine, so clone() whatever you keep."""
+        import torch
+        nc, nn = self.counts()
+        a, b, c = self.device_ptrs()
+        dev = torch.device("cuda", self.device)
+        return (torch.as_tensor(_DeviceView(a, (nc, 16)), device=dev), torch.as_tensor(_DeviceView(b, (nc, 10)), device=dev),
+                torch.as_tensor(_DeviceView(c, (nn,)), device=dev))
+
     def counts(self):
         nc, nn = C.c_int64(0), C.c_int64(0)
         _lib.check(self.L.csv_result_counts(self.h, C.byref(nc), C.byref(nn)))
         return nc.value, nn.value
 
-    def fetch(self):
+    def fetch(self, out=None):
         nc, nn = self.counts()
-        cands = np.zeros(max(nc, 1), dtype=_abi.CAND_DTYPE)
-        genos = np.zeros(max(nc, 1), dtype=_abi.GENO_DTYPE)
-        names = np.zeros(max(nn, 1), dtype=np.int32)
+        if out is not None:
+            cands, genos, names = out
+        else:
+            cands = np.zeros(max(nc, 1), dtype=_abi.CAND_DTYPE)
+            genos = np.zeros(max(nc, 1), dtype=_abi.GENO_DTYPE)
+            names = np.zeros(max(nn, 1), dtype=np.int32)
         _lib.check(self.L.csv_fetch(self.h, cands.ctypes.data_as(C.c_void_p), genos.ctypes.data_as(C.c_void_p), C.c_int64(len(cands)),
                                     _abi.ptr(names), C.c_int64(len(names))))
         return cands[:nc], genos[:nc], names[:nn]
 
     # -- the reference-facing one-shot call: host columns in, host rows out --
-    def cluster(self, sigs, reads, type_mask=0x1F, out=None, grouped=False):
+    def cluster(self, sigs, reads, type_mask=0x1F, out=None, grouped=False, stream=None):
         """sigs: {type_name: dict(chrom,a,b,read_id[,c])}; reads: dict(chrom,start,end,read_id,is_primary).
         grouped=True: every dict holds rows grouped by contig and `contig_off` instead of `chrom`
         (_abi.group_by_contig; csv_cluster_host_grouped).
-        Returns (cands, genos, names) numpy arrays in the reference's emission order."""
+        Returns (cands, genos, names) numpy arrays in the reference's emission order.
+        When any dict holds device columns (torch CUDA tensors), the inputs go through upload(..., stream=stream) and
+        csv_cluster instead of csv_cluster_host; the records still come back to the host."""
+        if any(_abi.is_device_array(v) for cols in list(sigs.values()) + [reads] for v in (cols or {}).values()):
+            self.upload({k: v for k, v in sigs.items() if type_mask >> _abi.TYPE_IDS[k] & 1}, reads, grouped=grouped, stream=stream)
+            self.cluster_device(type_mask)
+            return self.fetch(out)
         arr = (_abi.csv_sig_cols * _abi.CSV_NTYPES)()
         offs = (C.POINTER(C.c_int64) * _abi.CSV_NTYPES)()
         keep = []
@@ -331,6 +397,13 @@ class Engine(object):
         a, b, c = C.c_void_p(), C.c_void_p(), C.c_void_p()
         _lib.check(self.L.csv_result_device_ptrs(self.h, C.byref(a), C.byref(b), C.byref(c)))
         return a.value, b.value, c.value
+
+
+class _DeviceView(object):
+    """__cuda_array_interface__ of an int32 array the library owns (torch.as_tensor makes a view of it, no copy)."""
+
+    def __init__(self, ptr, shape):
+        self.__cuda_array_interface__ = {"shape": tuple(shape), "typestr": "<i4", "data": (int(ptr or 0), False), "version": 2}
 
 
 def _pin_packet_method(self, packed):

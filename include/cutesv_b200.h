@@ -197,6 +197,29 @@ int csv_upload_reads_grouped(csv_ctx* ctx, const csv_reads_cols* host_cols, cons
  * Precondition (as for the reads table): one primary record per read name. */
 int csv_upload_alignments(csv_ctx* ctx, const csv_reads_cols* aln);
 
+/* ---- the same uploads from columns that already live in GPU memory (a PyTorch pipeline, a GPU aligner, another ctx's
+ * extraction) ----
+ * Every non-null column (and contig_off, n_contigs + 1 int64) must be device or managed memory on the ctx's device, as
+ * cudaPointerGetAttributes reports it; anything else is CSV_E_INVALID naming the column.  Host columns keep going through the
+ * calls above.  Counts limits, the "column c required for INS/INV/TRA" rule and n == 0 behave as in the host calls.
+ *   - Copy, not borrow: the columns are copied device-to-device into the ctx's own buffers, which csv_remap_read_ids /
+ *     csv_swap_ins_rows rewrite and captured CUDA graphs address.
+ *   - Stream order both ways, no host synchronisation: stream is the caller's producer stream (NULL = the legacy default
+ *     stream).  The copies wait for everything enqueued on it before the call, and it waits for the copies: the caller may
+ *     overwrite or free its buffers in stream order as soon as the call returns.
+ *   - Grouped calls: contig_off is read on the device only.  Offsets that do not start at 0, end at n and never decrease make
+ *     the next csv_cluster return CSV_E_INPUT; the rows then get contig 0 and nothing outside the given buffers is read or
+ *     written.  An upload of the same slot with valid offsets (or any other upload of it) clears the report.
+ *   - csv_upload_alignments_device checks the table's order like csv_upload_alignments and, like it, blocks until that check
+ *     is done (the copies are then complete too).
+ * csv_cluster waits for pending device uploads before its kernel chain, so a call on fresh device inputs of unchanged sizes
+ * replays its captured graph (see csv_graph_replays). */
+int csv_upload_sigs_device(csv_ctx* ctx, int svtype, const csv_sig_cols* dev_cols, void* stream);
+int csv_upload_reads_device(csv_ctx* ctx, const csv_reads_cols* dev_cols, void* stream);
+int csv_upload_sigs_grouped_device(csv_ctx* ctx, int svtype, const csv_sig_cols* dev_cols, const int64_t* contig_off, void* stream);
+int csv_upload_reads_grouped_device(csv_ctx* ctx, const csv_reads_cols* dev_cols, const int64_t* contig_off, void* stream);
+int csv_upload_alignments_device(csv_ctx* ctx, const csv_reads_cols* dev_cols, void* stream);
+
 /* Replaces process_process_sigs_type (sort + dedup, cuteSV:750-857) and the whole clustering
  * phase Pool(run_del|run_ins|run_inv|run_dup|run_tra) (cuteSV:1113-1199) including call_gt /
  * overlap_cover / assign_gt / cal_GL (cuteSV_genotype.py:33-173) for every contig at once.
