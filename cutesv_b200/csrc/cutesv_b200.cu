@@ -56,9 +56,16 @@ extern "C" int csv_version(void) { return 100; }
 // replayed while the counter still has the value it had at capture time.
 static std::atomic<uint64_t> g_alloc_epoch{1};
 
+// Owns its allocation: freed when the buffer is destroyed (the ctx's buffers by `delete c`, on the ctx's device) or moved over.
 struct DBuf {
     void* p = nullptr;
     size_t cap = 0;
+    DBuf() = default;
+    DBuf(const DBuf&) = delete;
+    DBuf& operator=(const DBuf&) = delete;
+    DBuf(DBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+    DBuf& operator=(DBuf&& o) noexcept { if (this != &o) { release(); std::swap(p, o.p); std::swap(cap, o.cap); } return *this; }
+    ~DBuf() { release(); }
     cudaError_t ensure(size_t bytes, bool zero_new = false) {
         if (bytes <= cap) return cudaSuccess;
         g_alloc_epoch.fetch_add(1);
@@ -100,51 +107,42 @@ struct ExtractState {
     bool appending = false;
     double per_record[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // largest yield of a packet so far: signatures per type [0..4], pieces [5] per alignment record
 };
-static void extract_release(ExtractState* x) {
-    for (int k = 0; k < 7; k++) { x->r[k].release(); x->s[k].release(); }
-    for (int k = 0; k <= CSV_NTYPES; k++) x->rec[k].release();
-    x->cigar_off.release(); x->sa_off.release(); x->cigar.release(); x->piece_off.release(); x->piece_cnt.release();
-    x->pieces.release(); x->counters.release();
-    if (x->h_counters) cudaFreeHost(x->h_counters);
-    x->h_counters = nullptr;
-}
 
 // Lanes: SV types are independent until the `order` stage, so their kernel chains run concurrently on
-// separate streams (one lane per SV type; DEL uses the ctx stream).
-// Each lane owns the scratch its chain mutates; the buffers are swapped into the ctx while the lane's
-// launches are being enqueued (see csv_cluster).
-struct LaneWork {
+// separate streams, one lane per SV type (lane t runs type t; lane 0's stream is the ctx stream).  With lanes off every type
+// runs on lane 0.  A lane owns its stream's launch state and the scratch its chain mutates; the chain's functions take it as
+// an argument.
+struct Lane {
     cudaStream_t stream = nullptr;
     cudaEvent_t ev_join = nullptr;
-    bool used = false;
+    bool used = false;                  // forked from ev_fork in the call being enqueued
+    bool prev_is_chain_kernel = false;  // the launch being enqueued directly follows a chain kernel on this stream
     DBuf keys_a, keys_b, vals_a, vals_b, hist, lb_status, big_list, giant_list, giant_arena;
-    DBuf boff, rec_a, rec_b, recc_a, recc_b, rest_list;   // partitioned INS/DEL front end, k_cluster_small's rest list
+    DBuf boff, rec_a, recc_a, rest_list;   // partitioned INS/DEL front end, k_cluster_small's rest list
     SmallWork small;
 };
+static constexpr int N_LANES = CSV_NTYPES;
+
+// Look-back ticket words of one family of calls, zeroed at the start of every call.  A TileSync's generation is
+// *epoch * LB_ORDINALS + ordinal; where the epoch stays 0, ordinals start at ord0 = 1 so that none equals a cleared status word.
+struct LbPool {
+    uint32_t* tickets = nullptr;
+    const uint32_t* epoch = nullptr;
+    uint32_t ord0 = 0;
+    int next = 0, cap = 0;
+};
+
 // scratch of csv_overlap_cover / csv_call_gt (genotype_api.inl): separate from everything csv_cluster uses
 struct GcWork {
     DBuf win, bin_base, bin_start, bin_fill, bin_list, iter, prim, cov_off, ovl_off, cov_fill, ovl_fill, cov_u, ovl_u, lb, words;
     DBuf r_chrom, r_start, r_end, r_id, r_prim, cov_raw, ovl_raw, cov_ded, ovl_ded, cov_flag, ovl_flag, sup_off, sup, geno;
     uint32_t n_cov = 0, n_ovl = 0;   // raw ids of the last call
-    void release() {
-        DBuf* all[] = {&win, &bin_base, &bin_start, &bin_fill, &bin_list, &iter, &prim, &cov_off, &ovl_off, &cov_fill, &ovl_fill, &cov_u, &ovl_u,
-                       &lb, &words, &r_chrom, &r_start, &r_end, &r_id, &r_prim, &cov_raw, &ovl_raw, &cov_ded, &ovl_ded, &cov_flag, &ovl_flag,
-                       &sup_off, &sup, &geno};
-        for (DBuf* b : all) b->release();
-    }
 };
 
 // scratch of csv_sort_sigs (sigsort_api.inl): separate from everything csv_cluster uses
 struct SsWork {
     DBuf keys_a, keys_b, vals_a, vals_b, keep, tie, kchrom, order, off, hist, lb, words;
-    void release() {
-        DBuf* all[] = {&keys_a, &keys_b, &vals_a, &vals_b, &keep, &tie, &kchrom, &order, &off, &hist, &lb, &words};
-        for (DBuf* b : all) b->release();
-    }
 };
-
-static constexpr int N_LANES = CSV_NTYPES;
-static inline int lane_of(int t) { return t; }
 
 struct csv_ctx {
     int device = 0;
@@ -177,22 +175,17 @@ struct csv_ctx {
     DBuf r_chrom, r_start, r_end, r_id, r_prim;
     int64_t n_aln = 0;
     DBuf a_chrom, a_start, a_end, a_id, a_prim, a_off, a_span;
-    // sort workspace
-    DBuf keys_a, keys_b, vals_a, vals_b, hist, lb_status, tickets;
-    DBuf boff, rec_a, rec_b, recc_a, recc_b;   // partitioned INS/DEL front end (per lane, see LaneWork)
-    DBuf rest_list;                  // kept clusters k_cluster_small left to the general kernel (per lane)
-    DBuf scan_carry, emit_cursor;
+    DBuf tickets, scan_carry, emit_cursor;
     DBuf d_epoch;                    // look-back generation base, bumped by the first kernel of every csv_cluster
+    LbPool lb;                       // csv_cluster's look-back tickets, shared by its lanes (ordinals stay unique per call)
     uint32_t epoch_host = 0;
     bool small_chain[CSV_NTYPES] = {false, false, false, false, false};   // chained-sorts fallback after ST_BIG_RUN
     bool prefilter_enabled = true;
     bool records_enabled = true;
     bool small_path_enabled = true;
     int64_t pair_cap_override = 0;
-    int ticket_next = 0;
-    SmallWork small;
     DBuf d_goff[CSV_NTYPES + 1];   // contig row offsets of grouped uploads (last: reads table)
-    LaneWork lanes[N_LANES - 1];   // lane 0 = the ctx's own stream and buffers
+    Lane lanes[N_LANES];           // lanes[0].stream is `stream`
     cudaEvent_t ev_fork = nullptr;
     cudaStream_t side_stream[2] = {nullptr, nullptr};   // DEL / INS: the general cluster kernels beside the register kernel
     cudaEvent_t ev_side_fork[2] = {nullptr, nullptr}, ev_side_join[2] = {nullptr, nullptr};
@@ -200,7 +193,7 @@ struct csv_ctx {
     cudaEvent_t ev_aux = nullptr;
     bool lanes_enabled = true;
     // segment / cluster
-    DBuf kept[CSV_NTYPES], big_list, giant_list, giant_arena, cnt;
+    DBuf kept[CSV_NTYPES], cnt;
     uint32_t kept_cap[CSV_NTYPES] = {0, 0, 0, 0, 0};
     // results
     DBuf cand_tmp, cand, geno, names, counters;
@@ -212,9 +205,9 @@ struct csv_ctx {
     // state
     bool ran = false, counts_valid = false;
     int64_t launches = 0;
-    // profiling: CUDA-event intervals on the ctx stream; a stage may be entered once per SV type
+    // profiling: CUDA-event intervals on the launching streams; a stage may be entered once per SV type
     bool profiling = false;
-    struct Interval { int st; cudaEvent_t a, b; int64_t bytes; int dom_type; int64_t per_elem; };
+    struct Interval { int st; cudaEvent_t a, b; int64_t bytes; };
     std::vector<Interval> ivs;
     std::vector<cudaEvent_t> ev_pool;
     size_t ev_next = 0;
@@ -262,7 +255,6 @@ struct csv_ctx {
     bool pdl_now = false;               // ... for the call being enqueued: only with <= 2 SV-type lanes.  A dependent that is resident
                                         // early holds SM slots while it waits; with 5 lanes sharing the GPU those slots are what the
                                         // other lanes' kernels need
-    bool prev_is_chain_kernel = false;  // the launch being enqueued directly follows a chain kernel on the same stream
     DBuf cal_in0, cal_in1, cal_out, aln_flag;   // csv_cal_gl / csv_upload_alignments scratch (no per-call cudaMalloc)
     GcWork gc;                                  // csv_overlap_cover / csv_call_gt
     SsWork ss;                                  // csv_sort_sigs
@@ -272,46 +264,46 @@ struct csv_ctx {
     bool gathered = false;
 };
 
-static void kprof_begin(csv_ctx* c, const char* name);
-static void kprof_end(csv_ctx* c);
-// with profiling on, every launch sits between its own pair of CUDA events on the launching stream
-#define LAUNCH_NAMED(ctx, name, kernel, grid, block, smem, ...)                       \
+static void kprof_begin(csv_ctx* c, cudaStream_t s, const char* name);
+static void kprof_end(csv_ctx* c, cudaStream_t s);
+// with profiling on, every launch sits between its own pair of CUDA events on the launching stream `s`
+#define LAUNCH_NAMED(ctx, s, name, kernel, grid, block, smem, ...)                    \
     do {                                                                               \
-        if ((ctx)->profiling) kprof_begin((ctx), (name));                              \
-        kernel<<<(grid), (block), (smem), (ctx)->stream>>>(__VA_ARGS__);               \
-        if ((ctx)->profiling) kprof_end((ctx));                                        \
+        if ((ctx)->profiling) kprof_begin((ctx), (s), (name));                         \
+        kernel<<<(grid), (block), (smem), (s)>>>(__VA_ARGS__);                         \
+        if ((ctx)->profiling) kprof_end((ctx), (s));                                   \
         (ctx)->launches++;                                                             \
     } while (0)
-#define LAUNCH(ctx, kernel, grid, block, smem, ...) LAUNCH_NAMED(ctx, #kernel, kernel, grid, block, smem, __VA_ARGS__)
+#define LAUNCH(ctx, s, kernel, grid, block, smem, ...) LAUNCH_NAMED(ctx, s, #kernel, kernel, grid, block, smem, __VA_ARGS__)
 // A kernel that directly follows another kernel of the chain on the same stream (no copy, memset or join in between) and that
 // begins with pdl_wait(): launched as a programmatic dependent, so its launch latency and its CTAs' start-up overlap the tail
 // of its predecessor.  Captured into the CUDA graph as a programmatic edge.  Off when profiling (events sit between launches).
-#define LAUNCH_PDL_NAMED(ctx, name, kernel, grid, block, smem, ...)                                          \
+#define LAUNCH_PDL_NAMED(ctx, s, name, kernel, grid, block, smem, ...)                                       \
     do {                                                                                                      \
         if ((ctx)->pdl_now && !(ctx)->profiling) {                                                            \
             cudaLaunchConfig_t cfg_;                                                                          \
             memset(&cfg_, 0, sizeof(cfg_));                                                                   \
             cfg_.gridDim = dim3((unsigned)(grid)); cfg_.blockDim = dim3((unsigned)(block));                   \
-            cfg_.dynamicSmemBytes = (smem); cfg_.stream = (ctx)->stream;                                      \
+            cfg_.dynamicSmemBytes = (smem); cfg_.stream = (s);                                                \
             cudaLaunchAttribute at_[1];                                                                       \
             at_[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;                                   \
             at_[0].val.programmaticStreamSerializationAllowed = 1;                                            \
             cfg_.attrs = at_; cfg_.numAttrs = 1;                                                              \
             cudaLaunchKernelEx(&cfg_, kernel, __VA_ARGS__);                                                   \
             (ctx)->launches++;                                                                                \
-        } else LAUNCH_NAMED(ctx, name, kernel, grid, block, smem, __VA_ARGS__);                               \
+        } else LAUNCH_NAMED(ctx, s, name, kernel, grid, block, smem, __VA_ARGS__);                            \
     } while (0)
-#define LAUNCH_PDL(ctx, kernel, grid, block, smem, ...) LAUNCH_PDL_NAMED(ctx, #kernel, kernel, grid, block, smem, __VA_ARGS__)
+#define LAUNCH_PDL(ctx, s, kernel, grid, block, smem, ...) LAUNCH_PDL_NAMED(ctx, s, #kernel, kernel, grid, block, smem, __VA_ARGS__)
 
 // KIND: the per-type routine of the warp kernel (0 INS/DEL generic, 1 DUP, 2 INV, 3 TRA, 4-7 INS/DEL specialisations, see
 // run_cluster); the CTA kernel (rare big clusters) always uses the generic routine BKIND in 0..3
 template <int KIND, int BKIND>
-static void launch_cluster_kind(csv_ctx* c, const TypeJob& J, const Emit& E, Counters* ctr, uint32_t* work, size_t smem_warp) {
+static void launch_cluster_kind(csv_ctx* c, cudaStream_t s, const TypeJob& J, const Emit& E, Counters* ctr, uint32_t* work, size_t smem_warp) {
     static const char* const nm_w[8] = {"k_cluster_warp<INDEL>", "k_cluster_warp<DUP>", "k_cluster_warp<INV>", "k_cluster_warp<TRA>",
                                         "k_cluster_warp<DEL>", "k_cluster_warp<INS>", "k_cluster_warp<DEL,keep-all>", "k_cluster_warp<INS,keep-all>"};
     static const char* const nm_b[4] = {"k_cluster_block<INDEL>", "k_cluster_block<DUP>", "k_cluster_block<INV>", "k_cluster_block<TRA>"};
-    LAUNCH_NAMED(c, nm_w[KIND], (k_cluster_warp<KIND>), c->n_sm * 3, CL_THREADS, smem_warp, J, E, ctr, work);
-    LAUNCH_PDL_NAMED(c, nm_b[BKIND], (k_cluster_block<BKIND>), c->n_sm, CL_THREADS, (size_t)BLOCK_M * ARENA_PER_MAX, J, E, ctr);
+    LAUNCH_NAMED(c, s, nm_w[KIND], (k_cluster_warp<KIND>), c->n_sm * 3, CL_THREADS, smem_warp, J, E, ctr, work);
+    LAUNCH_PDL_NAMED(c, s, nm_b[BKIND], (k_cluster_block<BKIND>), c->n_sm, CL_THREADS, (size_t)BLOCK_M * ARENA_PER_MAX, J, E, ctr);
 }
 
 static int grid_for(const csv_ctx* c, int64_t n, int block, int per_sm = 8) {
@@ -352,26 +344,26 @@ static cudaEvent_t pool_event(csv_ctx* c) {
 static void stage_reset_if_consumed(csv_ctx* c) {
     if (c->ivs_consumed) { c->ivs.clear(); c->kivs.clear(); c->ev_next = 0; c->ivs_consumed = false; }
 }
-static void kprof_begin(csv_ctx* c, const char* name) {
+static void kprof_begin(csv_ctx* c, cudaStream_t s, const char* name) {
     stage_reset_if_consumed(c);
     csv_ctx::KInterval k;
     k.name = name; k.a = pool_event(c); k.b = pool_event(c);
-    cudaEventRecord(k.a, c->stream);
+    cudaEventRecord(k.a, s);
     c->kivs.push_back(k);
 }
-static void kprof_end(csv_ctx* c) { cudaEventRecord(c->kivs.back().b, c->stream); }
-static void stage_begin(csv_ctx* c, int st, int64_t bytes = 0, int dom_type = -1, int64_t per_elem = 0) {
+static void kprof_end(csv_ctx* c, cudaStream_t s) { cudaEventRecord(c->kivs.back().b, s); }
+static void stage_begin(csv_ctx* c, cudaStream_t s, int st, int64_t bytes = 0) {
     if (!c->profiling) return;
     stage_reset_if_consumed(c);
     csv_ctx::Interval iv;
-    iv.st = st; iv.a = pool_event(c); iv.b = pool_event(c); iv.bytes = bytes; iv.dom_type = dom_type; iv.per_elem = per_elem;
-    cudaEventRecord(iv.a, c->stream);
+    iv.st = st; iv.a = pool_event(c); iv.b = pool_event(c); iv.bytes = bytes;
+    cudaEventRecord(iv.a, s);
     c->ivs.push_back(iv);
 }
-static void stage_end(csv_ctx* c, int st) {
+static void stage_end(csv_ctx* c, cudaStream_t s, int st) {
     if (!c->profiling) return;
     for (size_t i = c->ivs.size(); i-- > 0;)
-        if (c->ivs[i].st == st) { cudaEventRecord(c->ivs[i].b, c->stream); return; }
+        if (c->ivs[i].st == st) { cudaEventRecord(c->ivs[i].b, s); return; }
 }
 static void stage_collect(csv_ctx* c) {  // after a stream synchronize
     for (int s = 0; s < CSV_ST_COUNT; s++) c->stage_ms[s] = 0.f;
@@ -379,11 +371,7 @@ static void stage_collect(csv_ctx* c) {  // after a stream synchronize
     for (const csv_ctx::Interval& iv : c->ivs) {
         float t = 0.f;
         if (cudaEventElapsedTime(&t, iv.a, iv.b) != cudaSuccess) { cudaGetLastError(); continue; }
-        if (iv.st == ST_SORT_PASS) {
-            int64_t bytes = iv.bytes;
-            if (iv.dom_type >= 0 && c->h_counters) bytes = (int64_t)c->h_counters->n_dom[iv.dom_type] * iv.per_elem;  // device-sized domain
-            c->sort_ms += t; c->sort_bytes += bytes; c->sort_launches++;
-        }
+        if (iv.st == ST_SORT_PASS) { c->sort_ms += t; c->sort_bytes += iv.bytes; c->sort_launches++; }
         else c->stage_ms[iv.st] += t;
     }
     c->ktotals.clear();
@@ -447,6 +435,7 @@ extern "C" int csv_create(int device, void* stream, csv_ctx** out) {
         if (e2 != cudaSuccess) { delete c; return set_err(CSV_E_CUDA, "cudaStreamCreate: %s", cudaGetErrorString(e2)); }
         c->own_stream = true;
     }
+    c->lanes[0].stream = c->stream;
     {
         cudaError_t e4 = cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking);
         for (int i = 0; i <= CSV_NTYPES && e4 == cudaSuccess; i++) e4 = cudaEventCreateWithFlags(&c->ev_up[i], cudaEventDisableTiming);
@@ -460,7 +449,7 @@ extern "C" int csv_create(int device, void* stream, csv_ctx** out) {
             if (e4 == cudaSuccess) e4 = cudaEventCreateWithFlags(&c->ev_side_fork[k], cudaEventDisableTiming);
             if (e4 == cudaSuccess) e4 = cudaEventCreateWithFlags(&c->ev_side_join[k], cudaEventDisableTiming);
         }
-        for (int l = 0; l < N_LANES - 1 && e4 == cudaSuccess; l++) {
+        for (int l = 1; l < N_LANES && e4 == cudaSuccess; l++) {   // lane 0 never joins: it is the ctx stream
             e4 = cudaStreamCreateWithFlags(&c->lanes[l].stream, cudaStreamNonBlocking);
             if (e4 == cudaSuccess) e4 = cudaEventCreateWithFlags(&c->lanes[l].ev_join, cudaEventDisableTiming);
         }
@@ -508,29 +497,13 @@ extern "C" int csv_destroy(csv_ctx* c) {
     if (!c) return CSV_OK;
     cudaSetDevice(c->device);
     cudaStreamSynchronize(c->stream);
-    DBuf* all[] = {&c->a_chrom, &c->a_start, &c->a_end, &c->a_id, &c->a_prim, &c->a_off, &c->a_span, &c->d_off, &c->d_len, &c->r_chrom, &c->r_start, &c->r_end, &c->r_id, &c->r_prim, &c->keys_a, &c->keys_b,
-                   &c->vals_a, &c->vals_b, &c->hist, &c->lb_status, &c->tickets, &c->big_list, &c->giant_list, &c->giant_arena,
-                   &c->cnt, &c->cand_tmp, &c->cand, &c->geno, &c->names, &c->counters, &c->bin_start, &c->bin_fill, &c->bin_bits, &c->pairs, &c->win_list,
-                   &c->dr, &c->has_rows, &c->gl_table, &c->pow_half, &c->small.k_rid, &c->small.k_b, &c->small.k_prim,
-                   &c->small.perm_a, &c->small.perm_b, &c->small.sel, &c->small.u_chrom, &c->small.u_a, &c->small.u_b,
-                   &c->small.u_rid, &c->small.u_c, &c->boff, &c->rec_a, &c->rec_b, &c->recc_a, &c->recc_b, &c->d_epoch,
-                   &c->d_len_eff, &c->g_send, &c->g_recv, &c->g_cand, &c->g_geno, &c->g_names, &c->g_scratch, &c->g_tab, &c->cal_in0, &c->cal_in1,
-                   &c->cal_out, &c->aln_flag, &c->scan_carry, &c->win_rec, &c->rest_list, &c->emit_cursor, &c->up_status};
-    for (DBuf* b : all) b->release();
-    c->gc.release();
-    c->ss.release();
     for (auto& g : c->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
     if (c->comm) comm_destroy(c);
     if (c->h_gather) cudaFreeHost(c->h_gather);
-    for (int l = 0; l < N_LANES - 1; l++) {
-        LaneWork& L = c->lanes[l];
+    for (int l = 1; l < N_LANES; l++) {
+        Lane& L = c->lanes[l];
         if (L.stream) { cudaStreamSynchronize(L.stream); cudaStreamDestroy(L.stream); }
         if (L.ev_join) cudaEventDestroy(L.ev_join);
-        DBuf* lb[] = {&L.keys_a, &L.keys_b, &L.vals_a, &L.vals_b, &L.hist, &L.lb_status, &L.big_list, &L.giant_list, &L.giant_arena,
-                      &L.boff, &L.rec_a, &L.rec_b, &L.recc_a, &L.recc_b, &L.rest_list,
-                      &L.small.k_rid, &L.small.k_b, &L.small.k_prim, &L.small.perm_a, &L.small.perm_b, &L.small.sel, &L.small.u_chrom, &L.small.u_a,
-                      &L.small.u_b, &L.small.u_rid, &L.small.u_c};
-        for (DBuf* b : lb) b->release();
     }
     if (c->ev_fork) cudaEventDestroy(c->ev_fork);
     if (c->aux_stream) { cudaStreamSynchronize(c->aux_stream); cudaStreamDestroy(c->aux_stream); }
@@ -540,12 +513,7 @@ extern "C" int csv_destroy(csv_ctx* c) {
         if (c->ev_side_fork[k]) cudaEventDestroy(c->ev_side_fork[k]);
         if (c->ev_side_join[k]) cudaEventDestroy(c->ev_side_join[k]);
     }
-    for (int i = 0; i <= CSV_NTYPES; i++) c->d_goff[i].release();
-    for (int t = 0; t < CSV_NTYPES; t++) {
-        c->sig[t].chrom.release(); c->sig[t].a.release(); c->sig[t].b.release(); c->sig[t].rid.release(); c->sig[t].c.release();
-        c->kept[t].release();
-    }
-    extract_release(&c->ex);
+    if (c->ex.h_counters) cudaFreeHost(c->ex.h_counters);
     for (cudaEvent_t e : c->ev_pool) cudaEventDestroy(e);
     if (c->h_counters) cudaFreeHost(c->h_counters);
     if (c->copy_stream) { cudaStreamSynchronize(c->copy_stream); cudaStreamDestroy(c->copy_stream); }
@@ -553,7 +521,7 @@ extern "C" int csv_destroy(csv_ctx* c) {
     if (c->ev_done) cudaEventDestroy(c->ev_done);
     if (c->ev_prod) cudaEventDestroy(c->ev_prod);
     if (c->own_stream) cudaStreamDestroy(c->stream);
-    delete c;
+    delete c;   // frees every device buffer (DBuf), on c->device
     return CSV_OK;
 }
 
@@ -690,9 +658,9 @@ static int upload_end(csv_ctx* c, int slot, const UpSrc& src) {
     c->up_device[slot] = src.device;
     return CSV_OK;
 }
-static int wait_upload(csv_ctx* c, int slot) {
+static int wait_upload(csv_ctx* c, cudaStream_t s, int slot) {
     if (c->up_pending[slot]) {
-        CU(cudaStreamWaitEvent(c->stream, c->ev_up[slot], 0));
+        CU(cudaStreamWaitEvent(s, c->ev_up[slot], 0));
         c->up_pending[slot] = false;
     }
     return CSV_OK;
@@ -848,9 +816,9 @@ static int upload_alignments_impl(csv_ctx* c, const csv_reads_cols* h, const UpS
     uint32_t* flag = c->aln_flag.as<uint32_t>();
     CU(cudaMemsetAsync(flag, 0, 4, c->stream));
     CU(cudaMemsetAsync(c->a_span.p, 0, ((size_t)c->n_contigs + 2) * 4, c->stream));
-    LAUNCH(c, k_aln_index, grid_for(c, h->n, 256), 256, 0, c->a_chrom.as<int32_t>(), c->a_start.as<int32_t>(), c->a_end.as<int32_t>(), h->n,
+    LAUNCH(c, c->stream, k_aln_index, grid_for(c, h->n, 256), 256, 0, c->a_chrom.as<int32_t>(), c->a_start.as<int32_t>(), c->a_end.as<int32_t>(), h->n,
            c->n_contigs, c->a_span.as<int32_t>(), flag);
-    LAUNCH(c, k_aln_off, grid_for(c, (int64_t)c->n_contigs + 1, 256), 256, 0, c->a_chrom.as<int32_t>(), h->n, c->n_contigs, c->a_off.as<uint32_t>());
+    LAUNCH(c, c->stream, k_aln_off, grid_for(c, (int64_t)c->n_contigs + 1, 256), 256, 0, c->a_chrom.as<int32_t>(), h->n, c->n_contigs, c->a_off.as<uint32_t>());
     uint32_t hflag = 0;
     CU(cudaMemcpyAsync(&hflag, flag, 4, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
@@ -868,55 +836,70 @@ extern "C" int csv_upload_alignments_device(csv_ctx* c, const csv_reads_cols* d,
 // ------------------------------------------------------------------------------------------
 // look-back sync objects
 // ------------------------------------------------------------------------------------------
-static int make_sync(csv_ctx* c, size_t status_words, TileSync* ts) {
-    if (c->ticket_next >= (int)LB_ORDINALS) return set_err(CSV_E_STATE, "ticket pool exhausted");
-    if (c->lb_status.cap < status_words * 8) {
-        CU(cudaStreamSynchronize(c->stream));
-        CU(c->lb_status.ensure(status_words * 8, true));
-    }
-    ts->ordinal = (uint32_t)c->ticket_next;
-    ts->ticket = c->tickets.as<uint32_t>() + c->ticket_next++;
-    ts->status = c->lb_status.as<uint64_t>();
-    ts->epoch = c->d_epoch.as<uint32_t>();
+// One ticket word of the pool, zero at the start of the call (a TileSync's, or a counter of a kernel chain)
+static int take_ticket(LbPool& lb, uint32_t** word) {
+    if (lb.next >= lb.cap) return set_err(CSV_E_STATE, "look-back ticket pool exhausted");
+    *word = lb.tickets + lb.next++;
     return CSV_OK;
+}
+// A TileSync over `status`, which must hold status_words words.  A status buffer that is too small grows, zero-filled, once
+// the work enqueued on `s` (which may still use it) is done.
+static int make_sync(LbPool& lb, DBuf& status, cudaStream_t s, size_t status_words, TileSync* ts) {
+    if (lb.next >= lb.cap) return set_err(CSV_E_STATE, "look-back ticket pool exhausted");
+    if (status.cap < status_words * 8) {
+        CU(cudaStreamSynchronize(s));
+        CU(status.ensure(status_words * 8, true));
+    }
+    ts->ordinal = lb.ord0 + (uint32_t)lb.next;
+    ts->status = status.as<uint64_t>();
+    ts->epoch = lb.epoch;
+    return take_ticket(lb, &ts->ticket);
 }
 
 // ------------------------------------------------------------------------------------------
-// radix sort driver: sorts (keys_a, vals_a) using (keys_b, vals_b) as the ping-pong partner.
-// vals_a == nullptr on input means "payload = iota".  Outputs point at the final buffers.
+// radix sort driver: sorts (keys_a, vals_a) using (keys_b, vals_b) as the ping-pong partner, on stream s with the
+// histogram buffer `hist` and look-back syncs from (lb, status).  iota: the payload of the first pass is the index.
+// probe: each pass is a csv_sort_probe interval.  Outputs point at the final buffers.
 // ------------------------------------------------------------------------------------------
 template <typename K>
-static int radix_sort(csv_ctx* c, K* keys_a, uint32_t* vals_a, K* keys_b, uint32_t* vals_b, bool iota, int64_t n,
-                      const uint32_t* n_dev, int bits, K** keys_out, uint32_t** vals_out, int dom_type = -1) {
+static int radix_sort(csv_ctx* c, cudaStream_t s, DBuf& hist, LbPool& lb, DBuf& status, bool probe, K* keys_a, uint32_t* vals_a,
+                      K* keys_b, uint32_t* vals_b, bool iota, int64_t n, int bits, K** keys_out, uint32_t** vals_out) {
+    const uint32_t* n_dev = nullptr;   // every sort's size is known on the host
     const int passes = std::max(1, (bits + 7) / 8);
     if (passes > RS_MAX_PASSES) return set_err(CSV_E_INVALID, "radix sort: %d bits", bits);
     constexpr int TILE = RS_THREADS * RsTraits<K>::ITEMS;
     const int64_t n_tiles = (n + TILE - 1) / TILE;
-    CU(c->hist.ensure(RS_MAX_PASSES * 256 * 4));
-    CU(cudaMemsetAsync(c->hist.p, 0, RS_MAX_PASSES * 256 * 4, c->stream));
-    LAUNCH(c, (k_rs_hist<K>), grid_for(c, n, RS_THREADS * 16, 4), RS_THREADS, 0, keys_a, n, n_dev, passes, c->hist.as<uint32_t>());
-    LAUNCH(c, k_rs_hist_scan, 1, 256, 0, c->hist.as<uint32_t>(), passes);
+    CU(hist.ensure(RS_MAX_PASSES * 256 * 4));
+    CU(cudaMemsetAsync(hist.p, 0, RS_MAX_PASSES * 256 * 4, s));
+    LAUNCH(c, s, (k_rs_hist<K>), grid_for(c, n, RS_THREADS * 16, 4), RS_THREADS, 0, keys_a, n, n_dev, passes, hist.as<uint32_t>());
+    LAUNCH(c, s, k_rs_hist_scan, 1, 256, 0, hist.as<uint32_t>(), passes);
     K* ki = keys_a; K* ko = keys_b;
     uint32_t* vi = vals_a; uint32_t* vo = vals_b;
     for (int p = 0; p < passes; p++) {
         TileSync ts;
-        int rc = make_sync(c, (size_t)n_tiles * 256, &ts);
+        int rc = make_sync(lb, status, s, (size_t)n_tiles * 256, &ts);
         if (rc) return rc;
         const int64_t per_elem = (int64_t)(sizeof(K) + ((p == 0 && iota) ? 0 : 4) + sizeof(K) + 4);
-        stage_begin(c, ST_SORT_PASS, n * per_elem, n_dev ? dom_type : -1, per_elem);
+        if (probe) stage_begin(c, s, ST_SORT_PASS, n * per_elem);
         if (p == 0 && iota)
-            LAUNCH(c, (k_rs_onesweep<K, true>), (int)n_tiles, RS_THREADS, 0, ki, (const uint32_t*)nullptr, ko, vo, n, n_dev, 8 * p,
-                   c->hist.as<uint32_t>() + p * 256, ts);
+            LAUNCH(c, s, (k_rs_onesweep<K, true>), (int)n_tiles, RS_THREADS, 0, ki, (const uint32_t*)nullptr, ko, vo, n, n_dev, 8 * p,
+                   hist.as<uint32_t>() + p * 256, ts);
         else
-            LAUNCH(c, (k_rs_onesweep<K, false>), (int)n_tiles, RS_THREADS, 0, ki, vi, ko, vo, n, n_dev, 8 * p,
-                   c->hist.as<uint32_t>() + p * 256, ts);
-        stage_end(c, ST_SORT_PASS);
+            LAUNCH(c, s, (k_rs_onesweep<K, false>), (int)n_tiles, RS_THREADS, 0, ki, vi, ko, vo, n, n_dev, 8 * p,
+                   hist.as<uint32_t>() + p * 256, ts);
+        if (probe) stage_end(c, s, ST_SORT_PASS);
         std::swap(ki, ko);
         std::swap(vi, vo);
     }
     *keys_out = ki;
     *vals_out = vi;
     return CSV_OK;
+}
+// csv_cluster's sorts: on lane L's stream and buffers, with the call's shared ticket pool
+template <typename K>
+static int lane_sort(csv_ctx* c, Lane& L, bool iota, int64_t n, int bits, K** keys_out, uint32_t** vals_out) {
+    return radix_sort<K>(c, L.stream, L.hist, c->lb, L.lb_status, true, L.keys_a.as<K>(), L.vals_a.as<uint32_t>(), L.keys_b.as<K>(),
+                         L.vals_b.as<uint32_t>(), iota, n, bits, keys_out, vals_out);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -949,19 +932,20 @@ static Emit make_emit(csv_ctx* c) {
     return E;
 }
 
-static int run_segment_and_cluster(csv_ctx* c, TypeJob& J, int t, uint32_t kslot_base) {
+static int run_segment_and_cluster(csv_ctx* c, Lane& L, TypeJob& J, int t, uint32_t kslot_base) {
     Counters* ctr = c->counters.as<Counters>();
+    const cudaStream_t s = L.stream;
     // ---- segment: kept chain clusters, in order ----
-    stage_begin(c, CSV_ST_SEGMENT);
+    stage_begin(c, s, CSV_ST_SEGMENT);
     J.kslot_base = kslot_base;
     J.kept_start = c->kept[t].as<uint32_t>();
-    J.big_list = c->big_list.as<uint32_t>();
-    J.giant_list = c->giant_list.as<uint32_t>();
-    J.giant_arena = c->giant_arena.as<char>();
-    J.big_cap = (uint32_t)(c->big_list.cap / 4);
-    J.giant_cap = (uint32_t)(c->giant_list.cap / 4);
+    J.big_list = L.big_list.as<uint32_t>();
+    J.giant_list = L.giant_list.as<uint32_t>();
+    J.giant_arena = L.giant_arena.as<char>();
+    J.big_cap = (uint32_t)(L.big_list.cap / 4);
+    J.giant_cap = (uint32_t)(L.giant_list.cap / 4);
     TileSync ts;
-    int rc = make_sync(c, (size_t)(J.n_host / SEL_TILE + 2), &ts);
+    int rc = make_sync(c->lb, L.lb_status, s, (size_t)(J.n_host / SEL_TILE + 2), &ts);
     if (rc) return rc;
     if ((J.cp.min_support + 31) / 32 + 1 <= HEAD_MAX_NEED_WORDS) {
         MemberRec MR;
@@ -971,78 +955,75 @@ static int run_segment_and_cluster(csv_ctx* c, TypeJob& J, int t, uint32_t kslot
             MR.rec = const_cast<IndelRec*>(J.iv.rec); MR.recc = const_cast<int32_t*>(J.iv.recc);
             MR.a = J.iv.a; MR.b = J.iv.b; MR.rid = J.iv.rid; MR.c = J.iv.recc ? J.iv.c : nullptr; MR.sidx = J.iv.sidx;
             if (J.cp.keep >= 1.0 && J.small_path) {   // the walk also sorts the kept clusters into the two lists of the cluster kernels
-                CU(c->rest_list.ensure((size_t)c->kept_cap[t] * 12 + 64));
-                if (c->ticket_next + 2 >= (int)LB_ORDINALS) return set_err(CSV_E_STATE, "ticket pool exhausted");
-                MR.rest_list = c->rest_list.as<uint32_t>();
-                MR.small_list = (uint2*)(c->rest_list.as<uint32_t>() + c->kept_cap[t] + (c->kept_cap[t] & 1u));
-                MR.n_small = c->tickets.as<uint32_t>() + c->ticket_next++;
-                MR.n_rest = c->tickets.as<uint32_t>() + c->ticket_next++;
+                CU(L.rest_list.ensure((size_t)c->kept_cap[t] * 12 + 64));
+                MR.rest_list = L.rest_list.as<uint32_t>();
+                MR.small_list = (uint2*)(L.rest_list.as<uint32_t>() + c->kept_cap[t] + (c->kept_cap[t] & 1u));
+                if ((rc = take_ticket(c->lb, &MR.n_small)) || (rc = take_ticket(c->lb, &MR.n_rest))) return rc;
                 J.small_list = MR.small_list; J.n_small = MR.n_small; J.rest_list = MR.rest_list; J.n_rest = MR.n_rest;
             }
         }
-        if (c->prev_is_chain_kernel)   // directly behind k_part_filter on this stream
-            LAUNCH_PDL(c, k_select_heads, grid_for(c, J.n_host, SEL_TILE, 4), SEL_THREADS, 0, J, c->kept[t].as<uint32_t>(), c->kept_cap[t],
+        if (L.prev_is_chain_kernel)   // directly behind k_part_filter on this stream
+            LAUNCH_PDL(c, s, k_select_heads, grid_for(c, J.n_host, SEL_TILE, 4), SEL_THREADS, 0, J, c->kept[t].as<uint32_t>(), c->kept_cap[t],
                        &ctr->n_kept[t], ts, &ctr->status, (uint32_t)ST_LIST_OVERFLOW, MR);
         else
-            LAUNCH(c, k_select_heads, grid_for(c, J.n_host, SEL_TILE, 4), SEL_THREADS, 0, J, c->kept[t].as<uint32_t>(), c->kept_cap[t],
+            LAUNCH(c, s, k_select_heads, grid_for(c, J.n_host, SEL_TILE, 4), SEL_THREADS, 0, J, c->kept[t].as<uint32_t>(), c->kept_cap[t],
                    &ctr->n_kept[t], ts, &ctr->status, (uint32_t)ST_LIST_OVERFLOW, MR);
     } else {
         J.iv.rec = nullptr; J.iv.recc = nullptr;   // generic path: members are gathered by the cluster kernels
         HeadPred hp{J};
-        LAUNCH(c, (k_select<HeadPred>), grid_for(c, J.n_host, SEL_TILE, 4), SEL_THREADS, 0, hp, J.n_host, J.n_dev,
+        LAUNCH(c, s, (k_select<HeadPred>), grid_for(c, J.n_host, SEL_TILE, 4), SEL_THREADS, 0, hp, J.n_host, J.n_dev,
                c->kept[t].as<uint32_t>(), c->kept_cap[t], &ctr->n_kept[t], ts, &ctr->status, (uint32_t)ST_LIST_OVERFLOW);
     }
-    stage_end(c, CSV_ST_SEGMENT);
+    stage_end(c, s, CSV_ST_SEGMENT);
     // ---- cluster ----
-    stage_begin(c, CSV_ST_CLUSTER);
+    stage_begin(c, s, CSV_ST_CLUSTER);
     Emit E = make_emit(c);
     const size_t smem_warp = (size_t)(CL_THREADS / 32) * WARP_M * ARENA_PER_MAX + (CL_THREADS / 32) * 40 * 8;
-    if (c->ticket_next >= (int)LB_ORDINALS) return set_err(CSV_E_STATE, "ticket pool exhausted");
-    uint32_t* work = c->tickets.as<uint32_t>() + c->ticket_next++;  // zeroed per call
+    uint32_t* work = nullptr;   // zeroed per call
+    if ((rc = take_ticket(c->lb, &work))) return rc;
     const bool keep_all = J.cp.keep >= 1.0;
-    cudaStream_t side = nullptr;   // the general kernels' stream while the register kernel runs on the lane's own
+    const int side_k = t == CSV_INS ? 1 : 0;
+    cudaStream_t gs = s;   // the general kernels' stream: a side stream while the register kernel runs on the lane's own
     if (kind_of(t) == 0 && keep_all && J.small_path) {
-        if (c->ticket_next + 2 >= (int)LB_ORDINALS) return set_err(CSV_E_STATE, "ticket pool exhausted");
-        uint32_t* work_s = c->tickets.as<uint32_t>() + c->ticket_next++;
+        uint32_t* work_s = nullptr;
+        if ((rc = take_ticket(c->lb, &work_s))) return rc;
         TypeJob JS = J;
         uint32_t* n_rest = nullptr;
         if (!J.small_list) {   // gather mode: the register kernel sizes the clusters itself and lists the larger ones
-            CU(c->rest_list.ensure((size_t)c->kept_cap[t] * 12 + 64));
-            n_rest = c->tickets.as<uint32_t>() + c->ticket_next++;
-            JS.rest_list = c->rest_list.as<uint32_t>();
+            CU(L.rest_list.ensure((size_t)c->kept_cap[t] * 12 + 64));
+            if ((rc = take_ticket(c->lb, &n_rest))) return rc;
+            JS.rest_list = L.rest_list.as<uint32_t>();
             JS.n_rest = n_rest;
         } else if (!c->profiling) {
             // both lists exist already: fork, the general kernels run beside the register kernel
-            side = c->side_stream[t == CSV_INS ? 1 : 0];
-            CU(cudaEventRecord(c->ev_side_fork[t == CSV_INS ? 1 : 0], c->stream));
-            CU(cudaStreamWaitEvent(side, c->ev_side_fork[t == CSV_INS ? 1 : 0], 0));
+            gs = c->side_stream[side_k];
+            CU(cudaEventRecord(c->ev_side_fork[side_k], s));
+            CU(cudaStreamWaitEvent(gs, c->ev_side_fork[side_k], 0));
         }
-        if (t == CSV_INS) LAUNCH_PDL_NAMED(c, "k_cluster_small<INS>", (k_cluster_small<true>), c->n_sm * 6, 256, 0, JS, E, ctr, work_s, n_rest);
-        else LAUNCH_PDL_NAMED(c, "k_cluster_small<DEL>", (k_cluster_small<false>), c->n_sm * 6, 256, 0, JS, E, ctr, work_s, n_rest);
+        if (t == CSV_INS) LAUNCH_PDL_NAMED(c, s, "k_cluster_small<INS>", (k_cluster_small<true>), c->n_sm * 6, 256, 0, JS, E, ctr, work_s, n_rest);
+        else LAUNCH_PDL_NAMED(c, s, "k_cluster_small<DEL>", (k_cluster_small<false>), c->n_sm * 6, 256, 0, JS, E, ctr, work_s, n_rest);
         if (!J.small_list) { J.rest_list = JS.rest_list; J.n_rest = n_rest; }
     } else { J.small_list = nullptr; J.n_small = nullptr; J.rest_list = nullptr; J.n_rest = nullptr; }
-    cudaStream_t lane_stream = c->stream;
-    if (side) c->stream = side;
     switch (kind_of(t)) {   // one per-type routine per kernel instantiation (instruction-cache footprint)
         case 0:
-            if (t == CSV_DEL) { if (keep_all) launch_cluster_kind<6, 0>(c, J, E, ctr, work, smem_warp); else launch_cluster_kind<4, 0>(c, J, E, ctr, work, smem_warp); }
-            else { if (keep_all) launch_cluster_kind<7, 0>(c, J, E, ctr, work, smem_warp); else launch_cluster_kind<5, 0>(c, J, E, ctr, work, smem_warp); }
+            if (t == CSV_DEL) { if (keep_all) launch_cluster_kind<6, 0>(c, gs, J, E, ctr, work, smem_warp); else launch_cluster_kind<4, 0>(c, gs, J, E, ctr, work, smem_warp); }
+            else { if (keep_all) launch_cluster_kind<7, 0>(c, gs, J, E, ctr, work, smem_warp); else launch_cluster_kind<5, 0>(c, gs, J, E, ctr, work, smem_warp); }
             break;
-        case 1: launch_cluster_kind<1, 1>(c, J, E, ctr, work, smem_warp); break;
-        case 2: launch_cluster_kind<2, 2>(c, J, E, ctr, work, smem_warp); break;
-        default: launch_cluster_kind<3, 3>(c, J, E, ctr, work, smem_warp); break;
+        case 1: launch_cluster_kind<1, 1>(c, gs, J, E, ctr, work, smem_warp); break;
+        case 2: launch_cluster_kind<2, 2>(c, gs, J, E, ctr, work, smem_warp); break;
+        default: launch_cluster_kind<3, 3>(c, gs, J, E, ctr, work, smem_warp); break;
     }
-    if (side) {
-        c->stream = lane_stream;
-        CU(cudaEventRecord(c->ev_side_join[t == CSV_INS ? 1 : 0], side));
-        CU(cudaStreamWaitEvent(c->stream, c->ev_side_join[t == CSV_INS ? 1 : 0], 0));
+    if (gs != s) {
+        CU(cudaEventRecord(c->ev_side_join[side_k], gs));
+        CU(cudaStreamWaitEvent(s, c->ev_side_join[side_k], 0));
     }
-    stage_end(c, CSV_ST_CLUSTER);
+    stage_end(c, s, CSV_ST_CLUSTER);
     return CSV_OK;
 }
 
-static int run_indel(csv_ctx* c, int t, uint32_t kslot_base) {
+static int run_indel(csv_ctx* c, Lane& L, int t, uint32_t kslot_base) {
     SigBuf& s = c->sig[t];
+    const cudaStream_t st = L.stream;
     const int64_t n = s.n;
     const uint64_t total = c->contig_off[c->n_contigs];
     const int bits = bits_for(total);
@@ -1071,62 +1052,60 @@ static int run_indel(csv_ctx* c, int t, uint32_t kslot_base) {
         const int P = (int)(total >> W) + 1;
         const int n_chunks = (int)((n + PART_CHUNK - 1) / PART_CHUNK);
         const size_t cnt_words = (size_t)P * n_chunks, edge_words = (size_t)P * 2 * BKT_PAD;
-        stage_begin(c, CSV_ST_KEYS);
-        CU(c->boff.ensure((cnt_words + P + 1 + edge_words) * 4));   // counts per (partition, chunk) | partition bases | edges
-        uint32_t* cnt = c->boff.as<uint32_t>();
+        stage_begin(c, st, CSV_ST_KEYS);
+        CU(L.boff.ensure((cnt_words + P + 1 + edge_words) * 4));   // counts per (partition, chunk) | partition bases | edges
+        uint32_t* cnt = L.boff.as<uint32_t>();
         uint32_t* pbase = cnt + cnt_words;
         uint32_t* edge = pbase + P + 1;
         // the spill area of partitions whose survivors exceed the shared-memory stage; the member records use it later
-        CU(c->rec_a.ensure((size_t)n * sizeof(IndelRec)));
-        if (c->ticket_next >= (int)LB_ORDINALS) return set_err(CSV_E_STATE, "ticket pool exhausted");
-        uint32_t* done_ctr = c->tickets.as<uint32_t>() + c->ticket_next++;
-        CU(cudaMemsetAsync(edge, 0, edge_words * 4, c->stream));
+        CU(L.rec_a.ensure((size_t)n * sizeof(IndelRec)));
+        uint32_t* done_ctr = nullptr;
+        if ((rc = take_ticket(c->lb, &done_ctr))) return rc;
+        CU(cudaMemsetAsync(edge, 0, edge_words * 4, st));
         const int is_ins = t == CSV_INS ? 1 : 0;
         if ((((uintptr_t)s.chrom.p) | ((uintptr_t)s.a.p)) & 15)   // k_part_scatter loads both columns 16 B at a time
             return set_err(CSV_E_STATE, "signature columns are not 16 B aligned");
-        LAUNCH(c, k_part_count, n_chunks, 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), n, is_ins, ct, W, P, n_chunks, rb, cnt, edge,
+        LAUNCH(c, st, k_part_count, n_chunks, 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), n, is_ins, ct, W, P, n_chunks, rb, cnt, edge,
                &ctr->status);
-        LAUNCH_PDL(c, k_part_scan, P, 256, 0, cnt, n_chunks, P, pbase, done_ctr);
-        uint2* pairs = (uint2*)c->keys_a.p;   // 8 B per signature (ensure_lane_scratch)
-        LAUNCH_PDL(c, k_part_scatter, n_chunks, 256, ps_smem_bytes(), s.chrom.as<int32_t>(), s.a.as<int32_t>(), n, is_ins, ct, W, P, n_chunks,
+        LAUNCH_PDL(c, st, k_part_scan, P, 256, 0, cnt, n_chunks, P, pbase, done_ctr);
+        uint2* pairs = (uint2*)L.keys_a.p;   // 8 B per signature (ensure_lane_scratch)
+        LAUNCH_PDL(c, st, k_part_scatter, n_chunks, 256, ps_smem_bytes(), s.chrom.as<int32_t>(), s.a.as<int32_t>(), n, is_ins, ct, W, P, n_chunks,
                    (const uint32_t*)cnt, (const uint32_t*)pbase, pairs);
-        stage_end(c, CSV_ST_KEYS);
-        stage_begin(c, CSV_ST_SORT);
+        stage_end(c, st, CSV_ST_KEYS);
+        stage_begin(c, st, CSV_ST_SORT);
         TileSync ts;
-        rc = make_sync(c, (size_t)P, &ts);
+        rc = make_sync(c->lb, L.lb_status, st, (size_t)P, &ts);
         if (rc) return rc;
         uint32_t* n_pass = &ctr->n_dom[t];
         const size_t smem = pf_smem_bytes(W);
         const int g = std::min(P, resident_grid(c, k_part_filter, 256, smem));
-        LAUNCH_PDL(c, k_part_filter, g, 256, smem, (const uint2*)pairs, (const uint32_t*)pbase, P, W, rb, (uint32_t)J.cp.min_support,
-                   (const uint32_t*)edge, c->keys_b.as<uint32_t>(), c->vals_b.as<uint32_t>(), (uint2*)c->rec_a.p, n_pass, ts);
-        stage_end(c, CSV_ST_SORT);
+        LAUNCH_PDL(c, st, k_part_filter, g, 256, smem, (const uint2*)pairs, (const uint32_t*)pbase, P, W, rb, (uint32_t)J.cp.min_support,
+                   (const uint32_t*)edge, L.keys_b.as<uint32_t>(), L.vals_b.as<uint32_t>(), (uint2*)L.rec_a.p, n_pass, ts);
+        stage_end(c, st, CSV_ST_SORT);
         J.n_dev = n_pass;
-        J.keys32 = c->keys_b.as<uint32_t>();
-        sidx = c->vals_b.as<uint32_t>();
+        J.keys32 = L.keys_b.as<uint32_t>();
+        sidx = L.vals_b.as<uint32_t>();
     } else {
-    stage_begin(c, CSV_ST_KEYS);
-    if (!k64)
-        LAUNCH(c, (k_indel_keys<uint32_t>), grid_for(c, n, 256), 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), s.b.as<int32_t>(),
-               s.rid.as<int32_t>(), n, t == CSV_INS ? 1 : 0, ct, c->keys_a.as<uint32_t>(), &ctr->status);
-    else
-        LAUNCH(c, (k_indel_keys<uint64_t>), grid_for(c, n, 256), 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), s.b.as<int32_t>(),
-               s.rid.as<int32_t>(), n, t == CSV_INS ? 1 : 0, ct, c->keys_a.as<uint64_t>(), &ctr->status);
-    stage_end(c, CSV_ST_KEYS);
-    stage_begin(c, CSV_ST_SORT);
-    if (!k64) {
-        uint32_t* ko = nullptr;
-        rc = radix_sort<uint32_t>(c, c->keys_a.as<uint32_t>(), c->vals_a.as<uint32_t>(), c->keys_b.as<uint32_t>(),
-                                  c->vals_b.as<uint32_t>(), true, n, nullptr, bits, &ko, &sidx);
-        J.keys32 = ko;
-    } else {
-        uint64_t* ko = nullptr;
-        rc = radix_sort<uint64_t>(c, c->keys_a.as<uint64_t>(), c->vals_a.as<uint32_t>(), c->keys_b.as<uint64_t>(),
-                                  c->vals_b.as<uint32_t>(), true, n, nullptr, bits, &ko, &sidx);
-        J.keys64 = ko;
-    }
-    if (rc) return rc;
-    stage_end(c, CSV_ST_SORT);
+        stage_begin(c, st, CSV_ST_KEYS);
+        if (!k64)
+            LAUNCH(c, st, (k_indel_keys<uint32_t>), grid_for(c, n, 256), 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), s.b.as<int32_t>(),
+                   s.rid.as<int32_t>(), n, t == CSV_INS ? 1 : 0, ct, L.keys_a.as<uint32_t>(), &ctr->status);
+        else
+            LAUNCH(c, st, (k_indel_keys<uint64_t>), grid_for(c, n, 256), 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), s.b.as<int32_t>(),
+                   s.rid.as<int32_t>(), n, t == CSV_INS ? 1 : 0, ct, L.keys_a.as<uint64_t>(), &ctr->status);
+        stage_end(c, st, CSV_ST_KEYS);
+        stage_begin(c, st, CSV_ST_SORT);
+        if (!k64) {
+            uint32_t* ko = nullptr;
+            rc = lane_sort<uint32_t>(c, L, true, n, bits, &ko, &sidx);
+            J.keys32 = ko;
+        } else {
+            uint64_t* ko = nullptr;
+            rc = lane_sort<uint64_t>(c, L, true, n, bits, &ko, &sidx);
+            J.keys64 = ko;
+        }
+        if (rc) return rc;
+        stage_end(c, st, CSV_ST_SORT);
     }
     J.iv.chrom = s.chrom.as<int32_t>(); J.iv.a = s.a.as<int32_t>(); J.iv.b = s.b.as<int32_t>(); J.iv.rid = s.rid.as<int32_t>();
     J.iv.c = s.has_c ? s.c.as<int32_t>() : nullptr;
@@ -1134,23 +1113,24 @@ static int run_indel(csv_ctx* c, int t, uint32_t kslot_base) {
     if (!k64 && c->records_enabled && (J.cp.min_support + 31) / 32 + 1 <= HEAD_MAX_NEED_WORDS) {
         // record mode: k_select_heads gathers one contiguous 16 B record (+ c of INS) per member of a kept chain cluster
         const bool with_c = t == CSV_INS && s.has_c;
-        CU(c->rec_a.ensure((size_t)n * sizeof(IndelRec)));
-        if (with_c) CU(c->recc_a.ensure((size_t)n * 4));
-        J.iv.rec = c->rec_a.as<IndelRec>();
-        J.iv.recc = with_c ? c->recc_a.as<int32_t>() : nullptr;
+        CU(L.rec_a.ensure((size_t)n * sizeof(IndelRec)));
+        if (with_c) CU(L.recc_a.ensure((size_t)n * 4));
+        J.iv.rec = L.rec_a.as<IndelRec>();
+        J.iv.recc = with_c ? L.recc_a.as<int32_t>() : nullptr;
     }
     J.iv.is_ins = t == CSV_INS ? 1 : 0;
     J.small_path = c->small_path_enabled ? 1 : 0;
-    c->prev_is_chain_kernel = prefilter;
-    rc = run_segment_and_cluster(c, J, t, kslot_base);
-    c->prev_is_chain_kernel = false;
+    L.prev_is_chain_kernel = prefilter;
+    rc = run_segment_and_cluster(c, L, J, t, kslot_base);
+    L.prev_is_chain_kernel = false;
     return rc;
 }
 
-static int run_other(csv_ctx* c, int t, uint32_t kslot_base) {
+static int run_other(csv_ctx* c, Lane& L, int t, uint32_t kslot_base) {
     SigBuf& s = c->sig[t];
+    const cudaStream_t st = L.stream;
     const int64_t n = s.n;
-    SmallWork& w = c->small;
+    SmallWork& w = L.small;
     ContigTab ct{c->d_off.as<uint64_t>(), c->d_len_eff.as<int64_t>(), c->n_contigs};
     Counters* ctr = c->counters.as<Counters>();
     // primary key = (chr, a) | (chr, strand, a) | (chr1, chr2*4+type, a): value range sized from the contig count
@@ -1163,113 +1143,100 @@ static int run_other(csv_ctx* c, int t, uint32_t kslot_base) {
     const int prim_bits = 31 + bits_for(compact ? (uint64_t)n : hi_max);
     const int32_t* col_c = s.has_c ? s.c.as<int32_t>() : nullptr;
     const bool chain = c->small_chain[t];
-    uint64_t* k_prim = chain ? w.k_prim.as<uint64_t>() : c->keys_a.as<uint64_t>();
+    uint64_t* k_prim = chain ? w.k_prim.as<uint64_t>() : L.keys_a.as<uint64_t>();
     int rc;
-    stage_begin(c, CSV_ST_KEYS);
+    stage_begin(c, st, CSV_ST_KEYS);
     if (!compact) {
-        LAUNCH(c, (k_other_keys<false>), grid_for(c, n, 256), 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), s.b.as<int32_t>(),
+        LAUNCH(c, st, (k_other_keys<false>), grid_for(c, n, 256), 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), s.b.as<int32_t>(),
                s.rid.as<int32_t>(), col_c, n, t, ct, chain ? w.k_rid.as<uint32_t>() : (uint32_t*)nullptr, w.k_b.as<uint32_t>(), k_prim,
                &ctr->status);
     } else {
         // pair words -> sort -> flags at pair changes -> exclusive scan = ranks -> (rank, a) scattered back to input order
-        LAUNCH(c, (k_other_keys<true>), grid_for(c, n, 256), 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), s.b.as<int32_t>(),
+        LAUNCH(c, st, (k_other_keys<true>), grid_for(c, n, 256), 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), s.b.as<int32_t>(),
                s.rid.as<int32_t>(), col_c, n, t, ct, chain ? w.k_rid.as<uint32_t>() : (uint32_t*)nullptr, w.k_b.as<uint32_t>(),
-               c->keys_a.as<uint64_t>(), &ctr->status);
+               L.keys_a.as<uint64_t>(), &ctr->status);
         uint64_t* pair_sorted = nullptr;
         uint32_t* pair_perm = nullptr;
-        rc = radix_sort<uint64_t>(c, c->keys_a.as<uint64_t>(), c->vals_a.as<uint32_t>(), c->keys_b.as<uint64_t>(), c->vals_b.as<uint32_t>(),
-                                  true, n, nullptr, bits_for(hi_max), &pair_sorted, &pair_perm);
+        rc = lane_sort<uint64_t>(c, L, true, n, bits_for(hi_max), &pair_sorted, &pair_perm);
         if (rc) return rc;
         uint32_t* rank = w.sel.as<uint32_t>();   // free until the de-duplication below
-        LAUNCH(c, k_tra_pair_flags, grid_for(c, n, 256), 256, 0, (const uint64_t*)pair_sorted, n, rank);
+        LAUNCH(c, st, k_tra_pair_flags, grid_for(c, n, 256), 256, 0, (const uint64_t*)pair_sorted, n, rank);
         TileSync ts;
-        rc = make_sync(c, (size_t)(n / (SEL_THREADS * 4) + 2), &ts);
+        rc = make_sync(c->lb, L.lb_status, st, (size_t)(n / (SEL_THREADS * 4) + 2), &ts);
         if (rc) return rc;
-        LAUNCH(c, (k_scan_excl<4>), grid_for(c, n, SEL_THREADS * 4, 4), SEL_THREADS, 0, rank, n, (const uint32_t*)nullptr,
+        LAUNCH(c, st, (k_scan_excl<4>), grid_for(c, n, SEL_THREADS * 4, 4), SEL_THREADS, 0, rank, n, (const uint32_t*)nullptr,
                (const uint32_t*)nullptr, (uint32_t*)nullptr, ts);
         // k_prim may alias pair_sorted (keys_a), which is no longer read; pair_perm is a value buffer
-        LAUNCH(c, k_tra_compact_key, grid_for(c, n, 256), 256, 0, (const uint32_t*)pair_perm, (const uint32_t*)rank, s.a.as<int32_t>(), n,
+        LAUNCH(c, st, k_tra_compact_key, grid_for(c, n, 256), 256, 0, (const uint32_t*)pair_perm, (const uint32_t*)rank, s.a.as<int32_t>(), n,
                k_prim);
     }
-    stage_end(c, CSV_ST_KEYS);
-    stage_begin(c, CSV_ST_SORT);
+    stage_end(c, st, CSV_ST_KEYS);
+    stage_begin(c, st, CSV_ST_SORT);
     if (!chain) {
         // ONE sort on the primary key (<= 8 passes instead of 16), then (b, name) order inside runs of equal primary keys
         uint64_t* k64o = nullptr;
         uint32_t* perm = nullptr;
-        rc = radix_sort<uint64_t>(c, c->keys_a.as<uint64_t>(), c->vals_a.as<uint32_t>(), c->keys_b.as<uint64_t>(), c->vals_b.as<uint32_t>(),
-                                  true, n, nullptr, prim_bits, &k64o, &perm);
+        rc = lane_sort<uint64_t>(c, L, true, n, prim_bits, &k64o, &perm);
         if (rc) return rc;
-        LAUNCH(c, k_run_fixup, grid_for(c, n, 256), 256, 0, k64o, perm, n, s.b.as<int32_t>(), s.rid.as<int32_t>(), w.perm_b.as<uint32_t>(),
+        LAUNCH(c, st, k_run_fixup, grid_for(c, n, 256), 256, 0, k64o, perm, n, s.b.as<int32_t>(), s.rid.as<int32_t>(), w.perm_b.as<uint32_t>(),
                &ctr->status);
     } else {
-    // LSD over the fields of the reference's tuple sort key: name, then second coordinate, then primary
-    // (fallback after ST_BIG_RUN: a run of equal primary keys too long for the ranking kernel)
-    uint32_t *k32o = nullptr, *perm = nullptr;
-    LAUNCH(c, (k_gather_keys<uint32_t>), grid_for(c, n, 256), 256, 0, w.k_rid.as<uint32_t>(), (const uint32_t*)nullptr, n, c->keys_a.as<uint32_t>());
-    rc = radix_sort<uint32_t>(c, c->keys_a.as<uint32_t>(), c->vals_a.as<uint32_t>(), c->keys_b.as<uint32_t>(), c->vals_b.as<uint32_t>(),
-                                  true, n, nullptr, 31, &k32o, &perm);
-    if (rc) return rc;
-    CU(cudaMemcpyAsync(w.perm_a.p, perm, (size_t)n * 4, cudaMemcpyDeviceToDevice, c->stream));
-    LAUNCH(c, (k_gather_keys<uint32_t>), grid_for(c, n, 256), 256, 0, w.k_b.as<uint32_t>(), w.perm_a.as<uint32_t>(), n, c->keys_a.as<uint32_t>());
-    CU(cudaMemcpyAsync(c->vals_a.p, w.perm_a.p, (size_t)n * 4, cudaMemcpyDeviceToDevice, c->stream));
-    rc = radix_sort<uint32_t>(c, c->keys_a.as<uint32_t>(), c->vals_a.as<uint32_t>(), c->keys_b.as<uint32_t>(), c->vals_b.as<uint32_t>(),
-                              false, n, nullptr, 31, &k32o, &perm);
-    if (rc) return rc;
-    CU(cudaMemcpyAsync(w.perm_a.p, perm, (size_t)n * 4, cudaMemcpyDeviceToDevice, c->stream));
-    LAUNCH(c, (k_gather_keys<uint64_t>), grid_for(c, n, 256), 256, 0, w.k_prim.as<uint64_t>(), w.perm_a.as<uint32_t>(), n, c->keys_a.as<uint64_t>());
-    CU(cudaMemcpyAsync(c->vals_a.p, w.perm_a.p, (size_t)n * 4, cudaMemcpyDeviceToDevice, c->stream));
-    uint64_t* k64o = nullptr;
-    rc = radix_sort<uint64_t>(c, c->keys_a.as<uint64_t>(), c->vals_a.as<uint32_t>(), c->keys_b.as<uint64_t>(), c->vals_b.as<uint32_t>(),
-                              false, n, nullptr, prim_bits, &k64o, &perm);
-    if (rc) return rc;
-    CU(cudaMemcpyAsync(w.perm_b.p, perm, (size_t)n * 4, cudaMemcpyDeviceToDevice, c->stream));
+        // LSD over the fields of the reference's tuple sort key: name, then second coordinate, then primary
+        // (fallback after ST_BIG_RUN: a run of equal primary keys too long for the ranking kernel)
+        uint32_t *k32o = nullptr, *perm = nullptr;
+        LAUNCH(c, st, (k_gather_keys<uint32_t>), grid_for(c, n, 256), 256, 0, w.k_rid.as<uint32_t>(), (const uint32_t*)nullptr, n, L.keys_a.as<uint32_t>());
+        rc = lane_sort<uint32_t>(c, L, true, n, 31, &k32o, &perm);
+        if (rc) return rc;
+        CU(cudaMemcpyAsync(w.perm_a.p, perm, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
+        LAUNCH(c, st, (k_gather_keys<uint32_t>), grid_for(c, n, 256), 256, 0, w.k_b.as<uint32_t>(), w.perm_a.as<uint32_t>(), n, L.keys_a.as<uint32_t>());
+        CU(cudaMemcpyAsync(L.vals_a.p, w.perm_a.p, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
+        rc = lane_sort<uint32_t>(c, L, false, n, 31, &k32o, &perm);
+        if (rc) return rc;
+        CU(cudaMemcpyAsync(w.perm_a.p, perm, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
+        LAUNCH(c, st, (k_gather_keys<uint64_t>), grid_for(c, n, 256), 256, 0, w.k_prim.as<uint64_t>(), w.perm_a.as<uint32_t>(), n, L.keys_a.as<uint64_t>());
+        CU(cudaMemcpyAsync(L.vals_a.p, w.perm_a.p, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
+        uint64_t* k64o = nullptr;
+        rc = lane_sort<uint64_t>(c, L, false, n, prim_bits, &k64o, &perm);
+        if (rc) return rc;
+        CU(cudaMemcpyAsync(w.perm_b.p, perm, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
     }
-    stage_end(c, CSV_ST_SORT);
+    stage_end(c, st, CSV_ST_SORT);
     // exact-duplicate removal + materialise the sorted columns
-    stage_begin(c, CSV_ST_SEGMENT);
+    stage_begin(c, st, CSV_ST_SEGMENT);
     uint32_t* n_u = &ctr->n_dom[t];  // device-side size of the de-duplicated domain
     TileSync ts;
-    rc = make_sync(c, (size_t)(n / SEL_TILE + 2), &ts);
+    rc = make_sync(c->lb, L.lb_status, st, (size_t)(n / SEL_TILE + 2), &ts);
     if (rc) return rc;
     DedupPred dp{s.chrom.as<int32_t>(), s.a.as<int32_t>(), s.b.as<int32_t>(), s.rid.as<int32_t>(), col_c, w.perm_b.as<uint32_t>()};
-    LAUNCH(c, (k_select<DedupPred>), grid_for(c, n, SEL_TILE, 4), SEL_THREADS, 0, dp, n, (const uint32_t*)nullptr, w.sel.as<uint32_t>(),
+    LAUNCH(c, st, (k_select<DedupPred>), grid_for(c, n, SEL_TILE, 4), SEL_THREADS, 0, dp, n, (const uint32_t*)nullptr, w.sel.as<uint32_t>(),
            (uint32_t)n, n_u, ts, &ctr->status, (uint32_t)ST_INTERNAL);
-    LAUNCH(c, k_other_gather, grid_for(c, n, 256), 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), s.b.as<int32_t>(), s.rid.as<int32_t>(),
+    LAUNCH(c, st, k_other_gather, grid_for(c, n, 256), 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), s.b.as<int32_t>(), s.rid.as<int32_t>(),
            col_c, w.perm_b.as<uint32_t>(), w.sel.as<uint32_t>(), n_u, w.u_chrom.as<int32_t>(), w.u_a.as<int32_t>(), w.u_b.as<int32_t>(),
            w.u_rid.as<int32_t>(), w.u_c.as<int32_t>());
-    stage_end(c, CSV_ST_SEGMENT);
+    stage_end(c, st, CSV_ST_SEGMENT);
     TypeJob J;
     memset(&J, 0, sizeof(J));
     J.svtype = t; J.n_host = n; J.n_dev = n_u;
     J.cp = cluster_params(c->P, t);
     J.sv.chrom = w.u_chrom.as<int32_t>(); J.sv.a = w.u_a.as<int32_t>(); J.sv.b = w.u_b.as<int32_t>();
     J.sv.rid = w.u_rid.as<int32_t>(); J.sv.c = w.u_c.as<int32_t>();
-    return run_segment_and_cluster(c, J, t, kslot_base);
+    return run_segment_and_cluster(c, L, J, t, kslot_base);
 }
 
-static void lane_swap(csv_ctx* c, LaneWork& L) {
-    std::swap(c->stream, L.stream);
-    std::swap(c->keys_a, L.keys_a); std::swap(c->keys_b, L.keys_b); std::swap(c->vals_a, L.vals_a); std::swap(c->vals_b, L.vals_b);
-    std::swap(c->hist, L.hist); std::swap(c->lb_status, L.lb_status);
-    std::swap(c->big_list, L.big_list); std::swap(c->giant_list, L.giant_list); std::swap(c->giant_arena, L.giant_arena);
-    std::swap(c->boff, L.boff); std::swap(c->rec_a, L.rec_a); std::swap(c->rec_b, L.rec_b); std::swap(c->recc_a, L.recc_a);
-    std::swap(c->recc_b, L.recc_b); std::swap(c->rest_list, L.rest_list);
-    std::swap(c->small, L.small);
-}
-static int ensure_small(csv_ctx* c, size_t ns) {
-    SmallWork& w = c->small;
+// lane L's DUP / INV / TRA scratch, for chains over at most ns signatures
+static int ensure_small(Lane& L, size_t ns) {
+    SmallWork& w = L.small;
     CU(w.k_rid.ensure(ns * 4)); CU(w.k_b.ensure(ns * 4)); CU(w.k_prim.ensure(ns * 8)); CU(w.perm_a.ensure(ns * 4)); CU(w.perm_b.ensure(ns * 4));
     CU(w.sel.ensure(ns * 4)); CU(w.u_chrom.ensure(ns * 4)); CU(w.u_a.ensure(ns * 4)); CU(w.u_b.ensure(ns * 4)); CU(w.u_rid.ensure(ns * 4));
     CU(w.u_c.ensure(ns * 4));
     return CSV_OK;
 }
-// scratch of the lane currently swapped into the ctx, for chains over at most nm signatures
-static int ensure_lane_scratch(csv_ctx* c, size_t nm) {
-    CU(c->keys_a.ensure(nm * 8)); CU(c->keys_b.ensure(nm * 8)); CU(c->vals_a.ensure(nm * 4)); CU(c->vals_b.ensure(nm * 4));
-    CU(c->big_list.ensure((nm / WARP_M + 2) * 4));
-    CU(c->giant_list.ensure((nm / BLOCK_M + 2) * 4));
-    CU(c->giant_arena.ensure(nm * 2 * ARENA_PER_MAX + 256));
+// lane L's sort and cluster scratch, for chains over at most nm signatures
+static int ensure_lane_scratch(Lane& L, size_t nm) {
+    CU(L.keys_a.ensure(nm * 8)); CU(L.keys_b.ensure(nm * 8)); CU(L.vals_a.ensure(nm * 4)); CU(L.vals_b.ensure(nm * 4));
+    CU(L.big_list.ensure((nm / WARP_M + 2) * 4));
+    CU(L.giant_list.ensure((nm / BLOCK_M + 2) * 4));
+    CU(L.giant_arena.ensure(nm * 2 * ARENA_PER_MAX + 256));
     return CSV_OK;
 }
 
@@ -1282,26 +1249,19 @@ static int ensure_workspace(csv_ctx* c, uint32_t type_mask) {
         if (t >= CSV_INV) n_small_max = std::max(n_small_max, c->sig[t].n);
     }
     const size_t nm = (size_t)std::max<int64_t>(n_max, 1);
-    int rc0 = ensure_lane_scratch(c, nm);   // lane 0 can run every type (lanes disabled / profiling)
-    if (rc0) return rc0;
+    int rc = ensure_lane_scratch(c->lanes[0], nm);   // lane 0 can run every type (lanes disabled)
+    if (rc) return rc;
     if (c->lanes_enabled) {
-        for (int l = 1; l < N_LANES; l++) {
-            int64_t nl = 0;
-            for (int t = 0; t < CSV_NTYPES; t++)
-                if ((type_mask >> t & 1) && lane_of(t) == l) nl = std::max(nl, c->sig[t].n);
+        for (int t = 1; t < CSV_NTYPES; t++) {   // lane t runs type t
+            const int64_t nl = (type_mask >> t & 1) ? c->sig[t].n : 0;
             if (nl == 0) continue;
-            LaneWork& L = c->lanes[l - 1];
-            lane_swap(c, L);
-            int rcl = ensure_lane_scratch(c, (size_t)nl);
-            if (!rcl && l >= CSV_INV) rcl = ensure_small(c, (size_t)nl);
-            lane_swap(c, L);
-            if (rcl) return rcl;
+            if ((rc = ensure_lane_scratch(c->lanes[t], (size_t)nl))) return rc;
+            if (t >= CSV_INV && (rc = ensure_small(c->lanes[t], (size_t)nl))) return rc;
         }
     }
     CU(c->tickets.ensure(LB_ORDINALS * 4));
     CU(c->counters.ensure(sizeof(Counters)));
-    rc0 = ensure_small(c, (size_t)std::max<int64_t>(n_small_max, 1));
-    if (rc0) return rc0;
+    if ((rc = ensure_small(c->lanes[0], (size_t)std::max<int64_t>(n_small_max, 1)))) return rc;
     uint64_t kept_total = 0;
     const int ms = std::max(1, c->P.min_support);
     for (int t = 0; t < CSV_NTYPES; t++) {
@@ -1326,8 +1286,8 @@ static int ensure_workspace(csv_ctx* c, uint32_t type_mask) {
 }
 
 static int join_lanes(csv_ctx* c) {
-    for (int l = 0; l < N_LANES - 1; l++) {
-        LaneWork& L = c->lanes[l];
+    for (int l = 1; l < N_LANES; l++) {
+        Lane& L = c->lanes[l];
         if (!L.used) continue;
         CU(cudaEventRecord(L.ev_join, L.stream));
         CU(cudaStreamWaitEvent(c->stream, L.ev_join, 0));
@@ -1342,7 +1302,7 @@ static int enqueue_cluster(csv_ctx* c, uint32_t type_mask) {
     int rc;
     stage_reset_if_consumed(c);
     c->last_mask = type_mask;
-    c->ticket_next = 0;
+    c->lb = LbPool{c->tickets.as<uint32_t>(), c->d_epoch.as<uint32_t>(), 0, 0, (int)LB_ORDINALS};   // k_begin zeroes the tickets
     {
         int n_lanes = 0;
         for (int t = 0; t < CSV_NTYPES; t++) n_lanes += ((type_mask >> t & 1) && c->sig[t].n > 0) ? 1 : 0;
@@ -1350,14 +1310,14 @@ static int enqueue_cluster(csv_ctx* c, uint32_t type_mask) {
     }
     // fresh look-back generation, zeroed tickets and counters.  (The per-cluster row counts `cnt` need no clearing: every
     // kept-cluster slot below n_kept[t] is written by a cluster kernel and the order scans stop at n_kept[t].)
-    LAUNCH(c, k_begin, 1, 256, 0, c->d_epoch.as<uint32_t>(), c->tickets.as<uint32_t>(), (int)LB_ORDINALS, c->counters.as<uint32_t>(),
+    LAUNCH(c, c->stream, k_begin, 1, 256, 0, c->d_epoch.as<uint32_t>(), c->tickets.as<uint32_t>(), (int)LB_ORDINALS, c->counters.as<uint32_t>(),
            (int)(sizeof(Counters) / 4), c->emit_cursor.as<unsigned long long>());
     Counters* ctr = c->counters.as<Counters>();
     uint32_t kslot_base = 0;
     // fork: every lane's chain starts after the resets above; join before `order`
     const bool lanes = c->lanes_enabled;
     if (lanes) CU(cudaEventRecord(c->ev_fork, c->stream));
-    for (int l = 0; l < N_LANES - 1; l++) c->lanes[l].used = false;
+    for (Lane& L : c->lanes) L.used = false;
     // genotype-stage scratch (bin tables of the linear coordinate): sized and cleared now, beside the lanes
     const uint64_t total_len = c->contig_off[c->n_contigs];
     int geno_shift = 10;
@@ -1378,15 +1338,11 @@ static int enqueue_cluster(csv_ctx* c, uint32_t type_mask) {
     }
     for (int t = 0; t < CSV_NTYPES; t++) {
         if (!(type_mask >> t & 1) || c->sig[t].n == 0) continue;
-        LaneWork* L = (lanes && lane_of(t) > 0) ? &c->lanes[lane_of(t) - 1] : nullptr;
-        if (L) {
-            if (!L->used) { CU(cudaStreamWaitEvent(L->stream, c->ev_fork, 0)); L->used = true; }
-            lane_swap(c, *L);   // c->stream and the scratch buffers are the lane's until swapped back
-        }
-        rc = wait_upload(c, t);
-        if (!rc && c->up_checked[t]) LAUNCH(c, k_fold_status, 1, 32, 0, c->up_status.as<uint32_t>() + t, &ctr->status);
-        if (!rc) rc = (t == CSV_DEL || t == CSV_INS) ? run_indel(c, t, kslot_base) : run_other(c, t, kslot_base);
-        if (L) lane_swap(c, *L);
+        Lane& L = c->lanes[lanes ? t : 0];
+        if (&L != &c->lanes[0] && !L.used) { CU(cudaStreamWaitEvent(L.stream, c->ev_fork, 0)); L.used = true; }
+        rc = wait_upload(c, L.stream, t);
+        if (!rc && c->up_checked[t]) LAUNCH(c, L.stream, k_fold_status, 1, 32, 0, c->up_status.as<uint32_t>() + t, &ctr->status);
+        if (!rc) rc = (t == CSV_DEL || t == CSV_INS) ? run_indel(c, L, t, kslot_base) : run_other(c, L, t, kslot_base);
         if (rc) {   // the ctx stream must not run ahead of work already forked
             join_lanes(c);
             if (aux_used) cudaStreamWaitEvent(c->stream, c->ev_aux, 0);
@@ -1413,7 +1369,7 @@ static int enqueue_cluster(csv_ctx* c, uint32_t type_mask) {
     G.gl_table = c->gl_table.as<csv_geno>();
     G.genotype = c->P.genotype;
     // ---- order ----
-    stage_begin(c, CSV_ST_ORDER);
+    stage_begin(c, c->stream, CSV_ST_ORDER);
     {
         // exclusive scan of the per-cluster row counts, one short scan per SV type over the slots actually used
         // (n_kept[t] of kept_cap[t]), chained through a carry word
@@ -1424,38 +1380,38 @@ static int enqueue_cluster(csv_ctx* c, uint32_t type_mask) {
         for (int t = 0; t < CSV_NTYPES; t++) {
             if (!(type_mask >> t & 1) || c->sig[t].n == 0) continue;
             TileSync ts;
-            rc = make_sync(c, (size_t)(c->kept_cap[t] / SEL_TILE + 2), &ts);
+            rc = make_sync(c->lb, c->lanes[0].lb_status, c->stream, (size_t)(c->kept_cap[t] / SEL_TILE + 2), &ts);
             if (rc) return rc;
             if (prev >= 0)
-                LAUNCH_PDL(c, (k_scan_excl<8>), grid_for(c, std::max<int64_t>(c->kept_cap[t], 1), SEL_TILE, 2), SEL_THREADS, 0, c->cnt.as<uint32_t>() + kb,
+                LAUNCH_PDL(c, c->stream, (k_scan_excl<8>), grid_for(c, std::max<int64_t>(c->kept_cap[t], 1), SEL_TILE, 2), SEL_THREADS, 0, c->cnt.as<uint32_t>() + kb,
                            (int64_t)c->kept_cap[t], (const uint32_t*)&ctr->n_kept[t], (const uint32_t*)(carry + prev), carry + t, ts);
             else
-                LAUNCH(c, (k_scan_excl<8>), grid_for(c, std::max<int64_t>(c->kept_cap[t], 1), SEL_TILE, 2), SEL_THREADS, 0, c->cnt.as<uint32_t>() + kb,
+                LAUNCH(c, c->stream, (k_scan_excl<8>), grid_for(c, std::max<int64_t>(c->kept_cap[t], 1), SEL_TILE, 2), SEL_THREADS, 0, c->cnt.as<uint32_t>() + kb,
                        (int64_t)c->kept_cap[t], (const uint32_t*)&ctr->n_kept[t], (const uint32_t*)nullptr, carry + t, ts);
             kb += c->kept_cap[t];
             prev = t;
         }
         // final order; the same pass counts the genotype windows per bin
-        LAUNCH_PDL(c, k_permute, grid_for(c, c->cap_cand, 256, 4), 256, 0, c->cand_tmp.as<csv_cand>(), c->cnt.as<uint32_t>(), ctr, c->cap_cand,
+        LAUNCH_PDL(c, c->stream, k_permute, grid_for(c, c->cap_cand, 256, 4), 256, 0, c->cand_tmp.as<csv_cand>(), c->cnt.as<uint32_t>(), ctr, c->cap_cand,
                c->cand.as<csv_cand>(), G, c->emit_cursor.as<unsigned long long>());
     }
-    stage_end(c, CSV_ST_ORDER);
+    stage_end(c, c->stream, CSV_ST_ORDER);
     // ---- genotype ----
-    rc = wait_upload(c, CSV_NTYPES);
+    rc = wait_upload(c, c->stream, CSV_NTYPES);
     if (rc) return rc;
     if (c->up_checked[CSV_NTYPES] && c->n_reads > 0)
-        LAUNCH(c, k_fold_status, 1, 32, 0, c->up_status.as<uint32_t>() + CSV_NTYPES, &ctr->status);
-    stage_begin(c, CSV_ST_GENOTYPE);
+        LAUNCH(c, c->stream, k_fold_status, 1, 32, 0, c->up_status.as<uint32_t>() + CSV_NTYPES, &ctr->status);
+    stage_begin(c, c->stream, CSV_ST_GENOTYPE);
     {
         if (c->P.genotype) {
             TileSync ts;
             // 1024-bin tiles, one 128-bit access per thread: the scan of the (at most 2^20 + 2) bins is a latency chain,
             // many small tiles on all SMs finish it sooner than few wide ones
-            rc = make_sync(c, (size_t)((G.n_bins + 1) / (SEL_THREADS * 4) + 2), &ts);
+            rc = make_sync(c->lb, c->lanes[0].lb_status, c->stream, (size_t)((G.n_bins + 1) / (SEL_THREADS * 4) + 2), &ts);
             if (rc) return rc;
-            LAUNCH_PDL(c, (k_scan_excl<4>), grid_for(c, G.n_bins + 1, SEL_THREADS * 4, 4), SEL_THREADS, 0, G.bin_start, (int64_t)G.n_bins + 1,
+            LAUNCH_PDL(c, c->stream, (k_scan_excl<4>), grid_for(c, G.n_bins + 1, SEL_THREADS * 4, 4), SEL_THREADS, 0, G.bin_start, (int64_t)G.n_bins + 1,
                    (const uint32_t*)nullptr, (const uint32_t*)nullptr, (uint32_t*)nullptr, ts);
-            LAUNCH_PDL(c, (k_windows<1>), grid_for(c, c->cap_cand, 256, 4), 256, 0, G);
+            LAUNCH_PDL(c, c->stream, (k_windows<1>), grid_for(c, c->cap_cand, 256, 4), 256, 0, G);
             if (c->n_reads > 0) {
                 PairBuf PB;
                 PB.cap = (uint32_t)std::min<int64_t>(4 * c->n_reads + (1 << 20), (int64_t)1 << 30);
@@ -1465,26 +1421,26 @@ static int enqueue_cluster(csv_ctx* c, uint32_t type_mask) {
                 PB.pairs4 = c->pairs.as<uint4>();
                 PB.count = &ctr->n_windows;
                 if (G.lin32) {
-                    LAUNCH_PDL(c, (k_reads_pass<true>), std::min(grid_for(c, c->n_reads, 1024, 8), resident_grid(c, k_reads_pass<true>, 256, 0)), 256, 0, G, PB, c->r_chrom.as<int32_t>(), c->r_start.as<int32_t>(),
+                    LAUNCH_PDL(c, c->stream, (k_reads_pass<true>), std::min(grid_for(c, c->n_reads, 1024, 8), resident_grid(c, k_reads_pass<true>, 256, 0)), 256, 0, G, PB, c->r_chrom.as<int32_t>(), c->r_start.as<int32_t>(),
                            c->r_end.as<int32_t>(), c->r_id.as<int32_t>(), c->r_prim.as<uint8_t>(), c->n_reads, &ctr->status);
-                    LAUNCH_PDL(c, (k_pairs_test<true>), c->n_sm * 8, 256, 0, G, PB, c->r_chrom.as<int32_t>(), c->r_start.as<int32_t>(),
+                    LAUNCH_PDL(c, c->stream, (k_pairs_test<true>), c->n_sm * 8, 256, 0, G, PB, c->r_chrom.as<int32_t>(), c->r_start.as<int32_t>(),
                            c->r_end.as<int32_t>(), c->r_id.as<int32_t>());
                 } else {
-                    LAUNCH_PDL(c, (k_reads_pass<false>), std::min(grid_for(c, c->n_reads, 1024, 8), resident_grid(c, k_reads_pass<false>, 256, 0)), 256, 0, G, PB, c->r_chrom.as<int32_t>(), c->r_start.as<int32_t>(),
+                    LAUNCH_PDL(c, c->stream, (k_reads_pass<false>), std::min(grid_for(c, c->n_reads, 1024, 8), resident_grid(c, k_reads_pass<false>, 256, 0)), 256, 0, G, PB, c->r_chrom.as<int32_t>(), c->r_start.as<int32_t>(),
                            c->r_end.as<int32_t>(), c->r_id.as<int32_t>(), c->r_prim.as<uint8_t>(), c->n_reads, &ctr->status);
-                    LAUNCH_PDL(c, (k_pairs_test<false>), c->n_sm * 8, 256, 0, G, PB, c->r_chrom.as<int32_t>(), c->r_start.as<int32_t>(),
+                    LAUNCH_PDL(c, c->stream, (k_pairs_test<false>), c->n_sm * 8, 256, 0, G, PB, c->r_chrom.as<int32_t>(), c->r_start.as<int32_t>(),
                            c->r_end.as<int32_t>(), c->r_id.as<int32_t>());
                 }
             }
         }
-        LAUNCH_PDL(c, k_finalize, grid_for(c, c->cap_cand, 256, 4), 256, 0, G);
+        LAUNCH_PDL(c, c->stream, k_finalize, grid_for(c, c->cap_cand, 256, 4), 256, 0, G);
         if (c->P.genotype && c->n_aln > 0 && (type_mask >> CSV_TRA & 1) && c->sig[CSV_TRA].n > 0) {
             AlnView A{c->a_chrom.as<int32_t>(), c->a_start.as<int32_t>(), c->a_end.as<int32_t>(), c->a_id.as<int32_t>(), c->a_prim.as<uint8_t>(),
                       c->a_off.as<uint32_t>(), c->a_span.as<int32_t>(), c->d_len.as<int64_t>()};
-            LAUNCH(c, k_tra_genotype, c->n_sm * 8, 128, 0, G, A, c->P.bias_tra, c->P.gt_round);   // 4 warps per CTA, one warp per TRA candidate
+            LAUNCH(c, c->stream, k_tra_genotype, c->n_sm * 8, 128, 0, G, A, c->P.bias_tra, c->P.gt_round);   // 4 warps per CTA, one warp per TRA candidate
         }
     }
-    stage_end(c, CSV_ST_GENOTYPE);
+    stage_end(c, c->stream, CSV_ST_GENOTYPE);
     return CSV_OK;
 }
 
@@ -1501,8 +1457,7 @@ extern "C" int csv_cluster(csv_ctx* c, uint32_t type_mask) {
     if (++c->epoch_host >= (1u << 21)) {
         CU(cudaDeviceSynchronize());
         CU(cudaMemset(c->d_epoch.p, 0, 64));
-        if (c->lb_status.p) CU(cudaMemset(c->lb_status.p, 0, c->lb_status.cap));
-        for (int l = 0; l < N_LANES - 1; l++) if (c->lanes[l].lb_status.p) CU(cudaMemset(c->lanes[l].lb_status.p, 0, c->lanes[l].lb_status.cap));
+        for (Lane& L : c->lanes) if (L.lb_status.p) CU(cudaMemset(L.lb_status.p, 0, L.lb_status.cap));
         c->epoch_host = 1;
     }
     // A call whose inputs are already resident (no upload in flight) and that is not being profiled replays a
@@ -1512,7 +1467,7 @@ extern "C" int csv_cluster(csv_ctx* c, uint32_t type_mask) {
     // uploads keep their per-type waits, which let the H2D copies of later types overlap the kernels of earlier ones.
     bool pending = false;
     for (int t = 0; t <= CSV_NTYPES; t++) {
-        if (c->up_pending[t] && c->up_device[t]) { rc = wait_upload(c, t); if (rc) return rc; }
+        if (c->up_pending[t] && c->up_device[t]) { rc = wait_upload(c, c->stream, t); if (rc) return rc; }
         pending |= c->up_pending[t];
     }
     bool done = false;
@@ -1624,13 +1579,13 @@ extern "C" int csv_fetch(csv_ctx* c, csv_cand* cands, csv_geno* genos, int64_t c
     int rc = csv_result_counts(c, &nc, &nn);
     if (rc) return rc;
     if (nc > cap_cand || nn > cap_names) return set_err(CSV_E_CAPACITY, "need %lld candidates / %lld names", (long long)nc, (long long)nn);
-    stage_begin(c, CSV_ST_D2H);
+    stage_begin(c, c->stream, CSV_ST_D2H);
     if (nc) {
         CU(cudaMemcpyAsync(cands, c->cand.p, (size_t)nc * sizeof(csv_cand), cudaMemcpyDeviceToHost, c->stream));
         CU(cudaMemcpyAsync(genos, c->geno.p, (size_t)nc * sizeof(csv_geno), cudaMemcpyDeviceToHost, c->stream));
     }
     if (nn) CU(cudaMemcpyAsync(names, c->names.p, (size_t)nn * 4, cudaMemcpyDeviceToHost, c->stream));
-    stage_end(c, CSV_ST_D2H);
+    stage_end(c, c->stream, CSV_ST_D2H);
     CU(cudaStreamSynchronize(c->stream));
     if (c->profiling) stage_collect(c);
     return CSV_OK;
@@ -1690,7 +1645,7 @@ extern "C" int csv_cal_gl(csv_ctx* c, const int32_t* c0, const int32_t* c1, int6
     csv_geno* dg = c->cal_out.as<csv_geno>();
     CU(cudaMemcpyAsync(d0, c0, n * 4, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d1, c1, n * 4, cudaMemcpyHostToDevice, c->stream));
-    LAUNCH(c, k_cal_gl, grid_for(c, n, 256), 256, 0, d0, d1, n, c->gl_table.as<csv_geno>(), dg);
+    LAUNCH(c, c->stream, k_cal_gl, grid_for(c, n, 256), 256, 0, d0, d1, n, c->gl_table.as<csv_geno>(), dg);
     CU(cudaMemcpyAsync(out, dg, n * sizeof(csv_geno), cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     return CSV_OK;
