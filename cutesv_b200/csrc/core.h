@@ -1236,11 +1236,41 @@ CSV_HD uint32_t pf_count(const H& h, int k, int bp, const uint32_t* hl, const ui
     return k < 0 ? hl[-k - 1] : k >= bp ? hr[k - bp] : h(k);
 }
 
+// An interior strip: every window [b - rb, b + rb] of its buckets lies inside [0, bp) and reaches at most the neighbouring
+// strips (rb <= n), so it needs neither the halo nor a bounds test.
+CSV_HD bool pf_strip_interior(int b0, int n, int bp, int rb) { return rb <= n && b0 - rb >= 0 && b0 + n - 1 + rb < bp; }
+
+// pf_strip_flags of an interior strip.  hs(s, j) = h(b0 + s * n + j) for s = -1, 0, 1 and 0 <= j < n: the caller indexes
+// its histogram directly (k_part_filter's transposed histogram: word (j << 8) + thread + s).
+template <class HS>
+CSV_HD uint64_t pf_strip_flags_interior(const HS& hs, int n, int rb, uint32_t need, uint32_t* kept) {
+    uint32_t win = 0, sum = 0;
+#pragma unroll 1
+    for (int k = 1; k <= rb; k++) win += hs(-1, n - k);
+#pragma unroll 1
+    for (int k = 0; k <= rb && k < n; k++) win += hs(0, k);
+    if (rb == n) win += hs(1, 0);
+    uint64_t flags = 0;
+    for (int j = 0; j < n; j++) {
+        if (j) {   // in: bucket j + rb of this strip or the next; out: bucket j - rb - 1 of this strip or the previous
+            const int ka = j + rb, sa = ka >= n ? 1 : 0;
+            const int ks = j - rb - 1, ss = ks < 0 ? -1 : 0;
+            win += hs(sa, ka - sa * n) - hs(ss, ks - ss * n);
+        }
+        const uint32_t c = hs(0, j);
+        if (c > 0 && win >= need) { flags |= 1ull << j; sum += c; }
+    }
+    *kept = sum;
+    return flags;
+}
+
 // Keep flags of a strip (bit j: bucket b0 + j) by a sliding window sum: 2 * rb + 1 reads for the first bucket, two for
-// every later one.  *kept = signatures in the strip's kept buckets.
-template <class H>
-CSV_HD uint64_t pf_strip_flags(const H& h, int b0, int n, int bp, int rb, uint32_t need, const uint32_t* hl, const uint32_t* hr,
-                               uint32_t* kept) {
+// every later one.  *kept = signatures in the strip's kept buckets.  Interior strips take pf_strip_flags_interior over
+// hs (as above); the others test every read against the partition's ends.
+template <class H, class HS>
+CSV_HD uint64_t pf_strip_flags(const H& h, const HS& hs, int b0, int n, int bp, int rb, uint32_t need, const uint32_t* hl,
+                               const uint32_t* hr, uint32_t* kept) {
+    if (pf_strip_interior(b0, n, bp, rb)) return pf_strip_flags_interior(hs, n, rb, need, kept);
     uint32_t win = 0, sum = 0;
     for (int k = b0 - rb; k <= b0 + rb; k++) win += pf_count(h, k, bp, hl, hr);
     uint64_t flags = 0;
@@ -1252,6 +1282,13 @@ CSV_HD uint64_t pf_strip_flags(const H& h, int b0, int n, int bp, int rb, uint32
     }
     *kept = sum;
     return flags;
+}
+
+// The same with the strip read through h alone.
+template <class H>
+CSV_HD uint64_t pf_strip_flags(const H& h, int b0, int n, int bp, int rb, uint32_t need, const uint32_t* hl, const uint32_t* hr,
+                               uint32_t* kept) {
+    return pf_strip_flags(h, [&](int s, int j) -> uint32_t { return h(b0 + s * n + j); }, b0, n, bp, rb, need, hl, hr, kept);
 }
 
 // Exclusive offsets of a strip's kept buckets, the first at `base`: put(j, offset, kept, count) for every bucket of the

@@ -1044,33 +1044,27 @@ static int run_indel(csv_ctx* c, Lane& L, int t, uint32_t kslot_base) {
     uint32_t* sidx = nullptr;
     int rc;
     if (prefilter) {
-        // filter-first front end, partitioned by genome range: count -> scan -> scatter of (key, index) by partition ->
-        // per partition, in shared memory: bucket histogram, density flags, survivors in key order.  W: the widest
-        // partitions (at most 2^22 bp) that still give every SM about two of them.
+        // filter-first front end, partitioned by genome range: scatter of (key, index) by partition inside every round of
+        // PART_ROUND rows -> per partition, in shared memory, over its runs: bucket histogram, density flags, survivors in
+        // key order.  W: the widest partitions (at most 2^22 bp) that still give every SM about two of them.
         int W = PART_W_MAX;
         while (W > PART_W_MIN && (int64_t)(total >> W) + 1 < 2 * (int64_t)c->n_sm) W--;
         const int P = (int)(total >> W) + 1;
-        const int n_chunks = (int)((n + PART_CHUNK - 1) / PART_CHUNK);
-        const size_t cnt_words = (size_t)P * n_chunks, edge_words = (size_t)P * 2 * BKT_PAD;
+        const int n_chunks = (int)((n + PART_ROUND - 1) / PART_ROUND);
+        const size_t run_words = (size_t)(P + 1) * n_chunks, edge_words = (size_t)P * 2 * BKT_PAD;
         stage_begin(c, st, CSV_ST_KEYS);
-        CU(L.boff.ensure((cnt_words + P + 1 + edge_words) * 4));   // counts per (partition, chunk) | partition bases | edges
-        uint32_t* cnt = L.boff.as<uint32_t>();
-        uint32_t* pbase = cnt + cnt_words;
-        uint32_t* edge = pbase + P + 1;
+        CU(L.boff.ensure((run_words + edge_words) * 4));   // run table (P + 1 rows of n_chunks) | edges
+        uint32_t* runs = L.boff.as<uint32_t>();
+        uint32_t* edge = runs + run_words;
         // the spill area of partitions whose survivors exceed the shared-memory stage; the member records use it later
         CU(L.rec_a.ensure((size_t)n * sizeof(IndelRec)));
-        uint32_t* done_ctr = nullptr;
-        if ((rc = take_ticket(c->lb, &done_ctr))) return rc;
         CU(cudaMemsetAsync(edge, 0, edge_words * 4, st));
         const int is_ins = t == CSV_INS ? 1 : 0;
         if ((((uintptr_t)s.chrom.p) | ((uintptr_t)s.a.p)) & 15)   // k_part_scatter loads both columns 16 B at a time
             return set_err(CSV_E_STATE, "signature columns are not 16 B aligned");
-        LAUNCH(c, st, k_part_count, n_chunks, 256, 0, s.chrom.as<int32_t>(), s.a.as<int32_t>(), n, is_ins, ct, W, P, n_chunks, rb, cnt, edge,
-               &ctr->status);
-        LAUNCH_PDL(c, st, k_part_scan, P, 256, 0, cnt, n_chunks, P, pbase, done_ctr);
         uint2* pairs = (uint2*)L.keys_a.p;   // 8 B per signature (ensure_lane_scratch)
-        LAUNCH_PDL(c, st, k_part_scatter, n_chunks, 256, ps_smem_bytes(), s.chrom.as<int32_t>(), s.a.as<int32_t>(), n, is_ins, ct, W, P, n_chunks,
-                   (const uint32_t*)cnt, (const uint32_t*)pbase, pairs);
+        LAUNCH(c, st, k_part_scatter, n_chunks, 256, ps_smem_bytes(), s.chrom.as<int32_t>(), s.a.as<int32_t>(), n, is_ins, ct, W, P,
+               n_chunks, rb, pairs, runs, edge, &ctr->status);
         stage_end(c, st, CSV_ST_KEYS);
         stage_begin(c, st, CSV_ST_SORT);
         TileSync ts;
@@ -1079,7 +1073,7 @@ static int run_indel(csv_ctx* c, Lane& L, int t, uint32_t kslot_base) {
         uint32_t* n_pass = &ctr->n_dom[t];
         const size_t smem = pf_smem_bytes(W);
         const int g = std::min(P, resident_grid(c, k_part_filter, 256, smem));
-        LAUNCH_PDL(c, st, k_part_filter, g, 256, smem, (const uint2*)pairs, (const uint32_t*)pbase, P, W, rb, (uint32_t)J.cp.min_support,
+        LAUNCH_PDL(c, st, k_part_filter, g, 256, smem, (const uint2*)pairs, (const uint32_t*)runs, n_chunks, P, W, rb, (uint32_t)J.cp.min_support,
                    (const uint32_t*)edge, L.keys_b.as<uint32_t>(), L.vals_b.as<uint32_t>(), (uint2*)L.rec_a.p, n_pass, ts);
         stage_end(c, st, CSV_ST_SORT);
         J.n_dev = n_pass;

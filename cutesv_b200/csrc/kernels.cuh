@@ -327,13 +327,12 @@ __device__ __forceinline__ uint32_t indel_key32(int32_t c, int32_t raw, int is_i
 // INS / DEL front end, partitioned: the genome's linear coordinate is cut into P partitions of 2^W bp (W <= 22, so a
 // partition has at most 16384 buckets of 256 bp).  The density filter then needs no genome-sized bucket table: every
 // partition's histogram is built, flagged, scanned and used inside one CTA's shared memory.
-//    k_part_count    8 B/sig read (chrom, a)          -> (partition, chunk) counts; halo counts at partition edges
-//    k_part_scan     4 B per (partition, chunk)       -> slot of every chunk inside every partition
-//    k_part_scatter  8 B/sig read, 8 B/sig written    -> (key, index) pairs grouped by partition
+//    k_part_scatter  8 B/sig read (chrom, a),        -> per round of PART_ROUND rows: its (key, index) pairs grouped by
+//                    8 B/sig written                    partition, written in place; the round's partition offsets (the
+//                                                       run table); halo counts at partition edges; input validation
 //    k_part_filter   8 B/sig read (twice, the second  -> survivors in key order, 8 B per survivor written
-//                    mostly from L2)
+//                    mostly from L2) + the run table
 // ------------------------------------------------------------------------------------------
-static constexpr int PART_CHUNK = 16384;     // signatures per CTA of k_part_count / k_part_scatter
 static constexpr int PART_MAX = 1024;        // partitions: 32-bit keys, W = 22
 static constexpr int PART_W_MAX = 22;
 static constexpr int PART_W_MIN = 16;        // >= 256 buckets per partition: the +-BKT_PAD halo reaches the neighbours only
@@ -344,165 +343,149 @@ __host__ __device__ constexpr size_t pf_smem_bytes(int w) {
     return (size_t)(1u << (w - BKT_SHIFT)) * 4 + (size_t)(1u << (w - BKT_SHIFT)) / 32 * 4 + (size_t)PF_STAGE * 8;
 }
 
-// One chunk of PART_CHUNK rows per CTA: f(key, row) for every row, with the same validation as k_indel_keys.
-template <class F>
-__device__ __forceinline__ void part_rows(const int32_t* __restrict__ chrom, const int32_t* __restrict__ a, int64_t n, int is_ins,
-                                          const ContigTab& ct, uint32_t& bad, F f) {
-    const int64_t c0 = (int64_t)blockIdx.x * PART_CHUNK;
-    const int64_t c1 = min(c0 + (int64_t)PART_CHUNK, n);
-    const bool aligned = ((((uintptr_t)chrom) | ((uintptr_t)a)) & 15) == 0;
-    const int64_t v1 = aligned ? (c1 >> 2) : (c0 >> 2);   // c0 is a multiple of 4
-    for (int64_t v = (c0 >> 2) + threadIdx.x; v < v1; v += blockDim.x) {
-        const int4 c4 = __ldcs(reinterpret_cast<const int4*>(chrom) + v), a4 = __ldcs(reinterpret_cast<const int4*>(a) + v);
-        f(indel_key32(c4.x, a4.x, is_ins, ct, bad), 4 * v);
-        f(indel_key32(c4.y, a4.y, is_ins, ct, bad), 4 * v + 1);
-        f(indel_key32(c4.z, a4.z, is_ins, ct, bad), 4 * v + 2);
-        f(indel_key32(c4.w, a4.w, is_ins, ct, bad), 4 * v + 3);
-    }
-    for (int64_t i = v1 * 4 + threadIdx.x; i < c1; i += blockDim.x) f(indel_key32(chrom[i], a[i], is_ins, ct, bad), i);
-}
-
-// cnt[p * n_chunks + chunk] = rows of the chunk in partition p.  edge[p][j] (j < BKT_PAD) counts the rows in the j-th
-// bucket of partition p, edge[p][BKT_PAD + j] those in its j-th bucket from the end: the halo of the neighbours' windows.
-__global__ void __launch_bounds__(256) k_part_count(const int32_t* __restrict__ chrom, const int32_t* __restrict__ a, int64_t n, int is_ins,
-                                                    ContigTab ct, int W, int P, int n_chunks, int rb, uint32_t* __restrict__ cnt,
-                                                    uint32_t* __restrict__ edge, uint32_t* status) {
-    pdl_launch_dependents();
-    __shared__ uint32_t s_c[PART_MAX];
-    for (int p = threadIdx.x; p < P; p += blockDim.x) s_c[p] = 0;
-    __syncthreads();
-    const uint32_t bmask = (1u << (W - BKT_SHIFT)) - 1;
-    uint32_t bad = 0;
-    part_rows(chrom, a, n, is_ins, ct, bad, [&](uint32_t key, int64_t) {
-        const uint32_t p = key >> W, bl = (key >> BKT_SHIFT) & bmask;
-        atomicAdd(&s_c[p], 1u);
-        if (bl < (uint32_t)rb) atomicAdd(&edge[p * 2 * BKT_PAD + bl], 1u);
-        if (bmask - bl < (uint32_t)rb) atomicAdd(&edge[p * 2 * BKT_PAD + BKT_PAD + (bmask - bl)], 1u);
-    });
-    if (bad) atomicOr(status, bad);
-    __syncthreads();
-    for (int p = threadIdx.x; p < P; p += blockDim.x) cnt[(int64_t)p * n_chunks + blockIdx.x] = s_c[p];
-}
-
-// One CTA per partition: its row of cnt becomes exclusive offsets inside the partition; the CTA that finishes last turns
-// the partition totals into partition bases: base[p] = first pair of partition p, base[P] = n.
-__global__ void __launch_bounds__(256) k_part_scan(uint32_t* __restrict__ cnt, int n_chunks, int P, uint32_t* __restrict__ base,
-                                                   uint32_t* done_ctr) {
-    pdl_launch_dependents(); pdl_wait();
-    __shared__ uint32_t s_warp[9];
-    __shared__ uint32_t s_last;
-    uint32_t* row = cnt + (int64_t)blockIdx.x * n_chunks;
-    uint32_t carry = 0;
-    for (int b = 0; b < n_chunks; b += 256) {
-        const int i = b + threadIdx.x;
-        const uint32_t v = i < n_chunks ? row[i] : 0u;
-        uint32_t total;
-        const uint32_t ex = block_excl_scan_256(v, s_warp, &total);
-        if (i < n_chunks) row[i] = carry + ex;
-        carry += total;
-    }
-    if (threadIdx.x == 0) base[blockIdx.x] = carry;
-    __threadfence();
-    if (threadIdx.x == 0) s_last = atomicAdd(done_ctr, 1u) == gridDim.x - 1 ? 1u : 0u;
-    __syncthreads();
-    if (!s_last) return;
-    __threadfence();
-    carry = 0;
-    for (int b = 0; b < P; b += 256) {
-        const int i = b + threadIdx.x;
-        const uint32_t v = i < P ? __ldcg(&base[i]) : 0u;
-        uint32_t total;
-        const uint32_t ex = block_excl_scan_256(v, s_warp, &total);
-        if (i < P) base[i] = carry + ex;
-        carry += total;
-    }
-    if (threadIdx.x == 0) base[P] = carry;
-}
-
-// (key, row) pairs grouped by partition; the order inside a partition is irrelevant (k_part_filter orders it).  The rows
-// of a chunk are grouped by partition in shared memory, PART_ROUND at a time, so that every partition's run is written with
-// coalesced stores: single 8 B stores scattered over a buffer larger than L2 end up as partial-sector writes to DRAM.  A
-// round of 8192 rows gives runs of about 11 pairs on permuted whole-genome input (P = 740); the stores of shorter runs
-// cost more than the loads.  A round issues all of its loads (16 B per column and thread, 8 of each) before the first key
-// is formed: the loads are the latency the kernel waits on, one round trip per round.  `chrom` and `a` must be 16 B
-// aligned (run_indel checks it); only the last 4-row group of the input is loaded row by row.
-static constexpr int PART_ROUND = 8192, PART_ROUND_V = PART_ROUND / 4 / 256;   // 4-row groups per thread and round
-static_assert(PART_CHUNK % PART_ROUND == 0 && PART_MAX == 4 * 256, "k_part_scatter tiling");
-__host__ __device__ constexpr size_t ps_smem_bytes() { return (size_t)PART_ROUND * 8 + (size_t)3 * PART_MAX * 4; }
+// One CTA per round of PART_ROUND rows (round c: rows c * PART_ROUND ..).  The round's (key, row) pairs are grouped by
+// partition in shared memory and written back in place, pairs[c * PART_ROUND + q], with coalesced 16 B stores: partition
+// p of round c is the run [runs[p * n_chunks + c], runs[(p + 1) * n_chunks + c]) of that block (row P of the run table
+// holds the round's row count).  The order inside a partition is irrelevant (k_part_filter orders it), and the filter
+// reads a partition as its list of runs, so no pass has to count the rows of every partition before they are written.
+// A round issues all of its loads (16 B per column and thread, 8 of each) before the first key is formed: the loads are
+// the latency the kernel waits on.  `chrom` and `a` must be 16 B aligned (run_indel checks it); only the last 4-row group
+// of the input is loaded row by row.  Rows in the first or last rb buckets of a partition are counted into edge[p][j]
+// (j < BKT_PAD: the j-th bucket of p; BKT_PAD + j: its j-th bucket from the end), the halo of the neighbours' windows.
+static constexpr int PART_ROUND = 8192, PART_ROUND_V = PART_ROUND / 4 / 256;   // 4-row groups per thread
+static_assert(PART_MAX == 4 * 256 && PART_ROUND < (1 << 14), "k_part_scatter tiling");
+__host__ __device__ constexpr size_t ps_smem_bytes() { return (size_t)PART_ROUND * 8 + (size_t)2 * PART_MAX * 4; }
 __global__ void __launch_bounds__(256) k_part_scatter(const int32_t* __restrict__ chrom, const int32_t* __restrict__ a, int64_t n, int is_ins,
-                                                      ContigTab ct, int W, int P, int n_chunks, const uint32_t* __restrict__ cnt,
-                                                      const uint32_t* __restrict__ base, uint2* __restrict__ pairs) {
-    pdl_launch_dependents(); pdl_wait();
+                                                      ContigTab ct, int W, int P, int n_chunks, int rb, uint2* __restrict__ pairs,
+                                                      uint32_t* __restrict__ runs, uint32_t* __restrict__ edge, uint32_t* status) {
+    pdl_launch_dependents();
     extern __shared__ __align__(16) uint32_t s_dyn[];
     uint2* s_st = reinterpret_cast<uint2*>(s_dyn);   // PART_ROUND pairs, grouped by partition
-    uint32_t* s_cur = s_dyn + 2 * PART_ROUND;        // next slot of every partition in `pairs`
-    uint32_t* s_off = s_cur + PART_MAX;              // rows of the round per partition -> their first position in s_st
+    uint32_t* s_off = s_dyn + 2 * PART_ROUND;        // rows of the round per partition -> their first position in s_st
     uint32_t* s_fill = s_off + PART_MAX;             // next free position of every partition in s_st
     __shared__ uint32_t s_warp[9];
-    for (int p = threadIdx.x; p < P; p += blockDim.x) s_cur[p] = base[p] + cnt[(int64_t)p * n_chunks + blockIdx.x];
-    const int64_t c1 = min((int64_t)(blockIdx.x + 1) * PART_CHUNK, n);
-    uint32_t dummy = 0;   // validated by k_part_count
-    for (int64_t s0 = (int64_t)blockIdx.x * PART_CHUNK; s0 < c1; s0 += PART_ROUND) {   // s0 is a multiple of 4
-        const int m = (int)min((int64_t)PART_ROUND, c1 - s0);
-        // No barrier between the last round's s_cur update and this clear: both loops give partition p to thread p % 256
-        // (the kernel runs with 256 threads), so a thread clears only the s_off words it has just read.
-        for (int p = threadIdx.x; p < PART_MAX; p += 256) s_off[p] = 0;
-        int4 cv[PART_ROUND_V], av[PART_ROUND_V];   // rows s0 + r .. s0 + r + 3, r = 4 * (j * 256 + thread)
+    const int64_t s0 = (int64_t)blockIdx.x * PART_ROUND;   // a multiple of 4
+    const int m = (int)min((int64_t)PART_ROUND, n - s0);
+    for (int p = threadIdx.x; p < PART_MAX; p += 256) s_off[p] = 0;
+    int4 cv[PART_ROUND_V], av[PART_ROUND_V];   // rows s0 + r .. s0 + r + 3, r = 4 * (j * 256 + thread)
 #pragma unroll
-        for (int j = 0; j < PART_ROUND_V; j++) {
-            const int r = 4 * (j * 256 + (int)threadIdx.x);
-            if (r + 4 <= m) {
-                cv[j] = __ldcs(reinterpret_cast<const int4*>(chrom + s0 + r));
-                av[j] = __ldcs(reinterpret_cast<const int4*>(a + s0 + r));
-            } else {
-                cv[j] = make_int4(r < m ? chrom[s0 + r] : 0, r + 1 < m ? chrom[s0 + r + 1] : 0, r + 2 < m ? chrom[s0 + r + 2] : 0,
-                                  r + 3 < m ? chrom[s0 + r + 3] : 0);
-                av[j] = make_int4(r < m ? a[s0 + r] : 0, r + 1 < m ? a[s0 + r + 1] : 0, r + 2 < m ? a[s0 + r + 2] : 0,
-                                  r + 3 < m ? a[s0 + r + 3] : 0);
+    for (int j = 0; j < PART_ROUND_V; j++) {
+        const int r = 4 * (j * 256 + (int)threadIdx.x);
+        if (r + 4 <= m) {
+            cv[j] = __ldcs(reinterpret_cast<const int4*>(chrom + s0 + r));
+            av[j] = __ldcs(reinterpret_cast<const int4*>(a + s0 + r));
+        } else {
+            cv[j] = make_int4(r < m ? chrom[s0 + r] : 0, r + 1 < m ? chrom[s0 + r + 1] : 0, r + 2 < m ? chrom[s0 + r + 2] : 0,
+                              r + 3 < m ? chrom[s0 + r + 3] : 0);
+            av[j] = make_int4(r < m ? a[s0 + r] : 0, r + 1 < m ? a[s0 + r + 1] : 0, r + 2 < m ? a[s0 + r + 2] : 0,
+                              r + 3 < m ? a[s0 + r + 3] : 0);
+        }
+    }
+    uint32_t key[4 * PART_ROUND_V], bad = 0;
+#pragma unroll
+    for (int j = 0; j < PART_ROUND_V; j++) {
+        const int r = 4 * (j * 256 + (int)threadIdx.x);
+        uint32_t b0 = 0, b1 = 0, b2 = 0, b3 = 0;   // rows past the input are not validated
+        key[4 * j] = indel_key32(cv[j].x, av[j].x, is_ins, ct, b0);
+        key[4 * j + 1] = indel_key32(cv[j].y, av[j].y, is_ins, ct, b1);
+        key[4 * j + 2] = indel_key32(cv[j].z, av[j].z, is_ins, ct, b2);
+        key[4 * j + 3] = indel_key32(cv[j].w, av[j].w, is_ins, ct, b3);
+        bad |= (r < m ? b0 : 0u) | (r + 1 < m ? b1 : 0u) | (r + 2 < m ? b2 : 0u) | (r + 3 < m ? b3 : 0u);
+    }
+    if (bad) atomicOr(status, bad);
+    const uint32_t bmask = (1u << (W - BKT_SHIFT)) - 1;
+#pragma unroll
+    for (int k = 0; k < 4 * PART_ROUND_V; k++) {
+        const uint32_t p = key[k] >> W, bl = (key[k] >> BKT_SHIFT) & bmask;
+        if (4 * ((k >> 2) * 256 + (int)threadIdx.x) + (k & 3) < m && (bl < (uint32_t)rb || bmask - bl < (uint32_t)rb)) {
+            if (bl < (uint32_t)rb) atomicAdd(&edge[p * 2 * BKT_PAD + bl], 1u);
+            if (bmask - bl < (uint32_t)rb) atomicAdd(&edge[p * 2 * BKT_PAD + BKT_PAD + (bmask - bl)], 1u);
+        }
+    }
+    __syncthreads();   // s_off cleared
+#pragma unroll
+    for (int k = 0; k < 4 * PART_ROUND_V; k++)
+        if (4 * ((k >> 2) * 256 + (int)threadIdx.x) + (k & 3) < m) atomicAdd(&s_off[key[k] >> W], 1u);
+    __syncthreads();
+    {   // exclusive scan of the per-partition counts, four partitions per thread; the run table gets rows 0..P-1
+        const uint4 v = reinterpret_cast<const uint4*>(s_off)[threadIdx.x];
+        uint32_t total;
+        const uint32_t ex = block_excl_scan_256(v.x + v.y + v.z + v.w, s_warp, &total);
+        const uint4 o = make_uint4(ex, ex + v.x, ex + v.x + v.y, ex + v.x + v.y + v.z);
+        reinterpret_cast<uint4*>(s_fill)[threadIdx.x] = o;
+        const int p0 = 4 * (int)threadIdx.x;
+        uint32_t* rc = runs + (int64_t)p0 * n_chunks + blockIdx.x;
+        if (p0 < P) rc[0] = o.x;
+        if (p0 + 1 < P) rc[n_chunks] = o.y;
+        if (p0 + 2 < P) rc[2 * (int64_t)n_chunks] = o.z;
+        if (p0 + 3 < P) rc[3 * (int64_t)n_chunks] = o.w;
+        if (threadIdx.x == 0) runs[(int64_t)P * n_chunks + blockIdx.x] = (uint32_t)m;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < 4 * PART_ROUND_V; k++) {
+        const int q = 4 * ((k >> 2) * 256 + (int)threadIdx.x) + (k & 3);
+        if (q < m) s_st[atomicAdd(&s_fill[key[k] >> W], 1u)] = make_uint2(key[k], (uint32_t)(s0 + q));
+    }
+    __syncthreads();
+    uint2* dst = pairs + s0;   // 16 B aligned: s0 is a multiple of PART_ROUND
+    for (int q = threadIdx.x; q < (m >> 1); q += 256) reinterpret_cast<uint4*>(dst)[q] = reinterpret_cast<const uint4*>(s_st)[q];
+    if ((m & 1) && threadIdx.x == 0) dst[m - 1] = s_st[m - 1];
+}
+
+// f(pair, valid) for every pair of partition p, i.e. of the runs [c * PART_ROUND + runs[p][c], c * PART_ROUND +
+// runs[p + 1][c]) of the rounds c < n_chunks (k_part_scatter's run table, runs[p][c] at runs[p * n_chunks + c]).  Every
+// warp takes tiles of 32 consecutive runs, one per lane, in turn with the CTA's other warps (the next tile's run bounds are
+// loaded before the current one is walked).  A warp scan of the run lengths numbers the tile's pairs; the lane that takes
+// pair e finds its run by a five-step binary search over the lanes' run ends (shuffles: no shared memory, no per-pair
+// search in memory).  U pairs per lane are loaded before f sees the first.  f is called by every lane of the warp
+// together, `valid` false past the tile's last pair.
+template <int U, class F>
+__device__ __forceinline__ void part_walk_runs(const uint2* __restrict__ pairs, const uint32_t* __restrict__ runs, int p, int n_chunks,
+                                               F f) {
+    const int lane = threadIdx.x & 31;
+    const uint32_t* r0 = runs + (int64_t)p * n_chunks;
+    const uint32_t* r1 = r0 + n_chunks;
+    int c = (int)(threadIdx.x & ~31u) + lane;   // warp w starts at run 32 w
+    uint32_t nb = 0, ne = 0;
+    if (c < n_chunks) { nb = __ldcg(r0 + c); ne = __ldcg(r1 + c); }
+    for (; c - lane < n_chunks; c += 256) {
+        const uint32_t len = ne - nb;
+        uint32_t end = len;   // inclusive scan of the run lengths: the tile's pairs end[r - 1] .. end[r] - 1 are run r's
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint32_t v = __shfl_up_sync(0xffffffffu, end, d);
+            if (lane >= d) end += v;
+        }
+        const uint32_t tot = __shfl_sync(0xffffffffu, end, 31);
+        const uint32_t src = (uint32_t)c * PART_ROUND + nb - (end - len);   // pair e of the tile, in run r: pairs[src(r) + e]
+        nb = ne = 0;
+        if (c + 256 < n_chunks) { nb = __ldcg(r0 + c + 256); ne = __ldcg(r1 + c + 256); }
+        const uint32_t end15 = __shfl_sync(0xffffffffu, end, 15);   // the searches' first step
+        for (uint32_t e0 = 0; e0 < tot; e0 += 32 * U) {
+            uint32_t at[U];
+#pragma unroll
+            for (int u = 0; u < U; u++) {   // no branch around a search, so that the U searches interleave
+                const uint32_t e = e0 + 32 * u + lane;
+                int r = end15 <= e ? 16 : 0;
+#pragma unroll
+                for (int s = 8; s; s >>= 1) r += __shfl_sync(0xffffffffu, end, r + s - 1) <= e ? s : 0;
+                at[u] = __shfl_sync(0xffffffffu, src, r) + e;
             }
-        }
-        uint32_t key[4 * PART_ROUND_V];
+            uint2 pr[U];
 #pragma unroll
-        for (int j = 0; j < PART_ROUND_V; j++) {
-            key[4 * j] = indel_key32(cv[j].x, av[j].x, is_ins, ct, dummy);
-            key[4 * j + 1] = indel_key32(cv[j].y, av[j].y, is_ins, ct, dummy);
-            key[4 * j + 2] = indel_key32(cv[j].z, av[j].z, is_ins, ct, dummy);
-            key[4 * j + 3] = indel_key32(cv[j].w, av[j].w, is_ins, ct, dummy);
-        }
-        __syncthreads();   // s_off cleared; the previous round's stores have read s_st
+            for (int u = 0; u < U; u++) pr[u] = e0 + 32 * u + lane < tot ? pairs[at[u]] : make_uint2(0u, 0u);
 #pragma unroll
-        for (int k = 0; k < 4 * PART_ROUND_V; k++)
-            if (4 * ((k >> 2) * 256 + (int)threadIdx.x) + (k & 3) < m) atomicAdd(&s_off[key[k] >> W], 1u);
-        __syncthreads();
-        {   // exclusive scan of the per-partition counts, four partitions per thread
-            const uint4 v = reinterpret_cast<const uint4*>(s_off)[threadIdx.x];
-            uint32_t total;
-            const uint32_t ex = block_excl_scan_256(v.x + v.y + v.z + v.w, s_warp, &total);
-            const uint4 o = make_uint4(ex, ex + v.x, ex + v.x + v.y, ex + v.x + v.y + v.z);
-            reinterpret_cast<uint4*>(s_off)[threadIdx.x] = o;
-            reinterpret_cast<uint4*>(s_fill)[threadIdx.x] = o;
+            for (int u = 0; u < U; u++) f(pr[u], e0 + 32 * u + lane < tot);
         }
-        __syncthreads();
-#pragma unroll
-        for (int k = 0; k < 4 * PART_ROUND_V; k++) {
-            const int q = 4 * ((k >> 2) * 256 + (int)threadIdx.x) + (k & 3);
-            if (q < m) s_st[atomicAdd(&s_fill[key[k] >> W], 1u)] = make_uint2(key[k], (uint32_t)(s0 + q));
-        }
-        __syncthreads();
-        for (int q = threadIdx.x; q < m; q += 256) {
-            const uint2 pr = s_st[q];
-            const uint32_t p = pr.x >> W;
-            pairs[s_cur[p] + (uint32_t)q - s_off[p]] = pr;
-        }
-        __syncthreads();
-        for (int p = threadIdx.x; p < P; p += 256) s_cur[p] += s_fill[p] - s_off[p];   // same p -> thread map as the clear
     }
 }
 
 // One partition per CTA iteration (partitions taken by ticket, in order):
-//   1. 256-bp bucket histogram of the partition in shared memory
+//   1. 256-bp bucket histogram of the partition in shared memory, its pairs read as the run list of the scatter's rounds
 //   2. one pass over every thread's strip of BP / 256 consecutive buckets: keep flags by a sliding +-rb window (the halo
-//      taken from the neighbours' edge counts -- the same rule as a genome-wide histogram) and the strip's survivors;
+//      taken from the neighbours' edge counts -- the same rule as a genome-wide histogram; strips whose windows stay
+//      inside the partition and reach only the neighbouring strips skip the halo tests) and the strip's survivors;
 //      one CTA scan gives the partition's survivor total, published to the look-back at once, and every strip's base
 //   3. a second pass over the strip writes the exclusive offsets of the kept buckets and their flag bits; the pairs are
 //      streamed again and every survivor is put into its bucket's slot range in the shared-memory stage (more than
@@ -513,7 +496,7 @@ __global__ void __launch_bounds__(256) k_part_scatter(const int32_t* __restrict_
 // threads reading the j-th bucket of their strips touch 256 consecutive words.  The look-back's exclusive base is
 // awaited only where it is used: before the placement of a partition that spills, otherwise by warp 0 before its share
 // of the placement, while the other warps place theirs.
-__global__ void __launch_bounds__(256) k_part_filter(const uint2* __restrict__ pairs, const uint32_t* __restrict__ base, int P, int W, int rb,
+__global__ void __launch_bounds__(256) k_part_filter(const uint2* __restrict__ pairs, const uint32_t* __restrict__ runs, int n_chunks, int P, int W, int rb,
                                                      uint32_t need, const uint32_t* __restrict__ edge, uint32_t* __restrict__ keys_out,
                                                      uint32_t* __restrict__ idx_out, uint2* __restrict__ spill, uint32_t* n_out, TileSync ts) {
     pdl_launch_dependents(); pdl_wait();
@@ -545,22 +528,17 @@ __global__ void __launch_bounds__(256) k_part_filter(const uint2* __restrict__ p
             const bool ok = q >= 0 && q < P && j < rb;
             (right ? s_hr : s_hl)[j] = ok ? edge[(int64_t)q * 2 * BKT_PAD + (right ? 0 : BKT_PAD) + j] : 0u;
         }
-        const int64_t lo = base[p], cnt = (int64_t)base[p + 1] - lo;
-        const uint2* src_pairs = pairs + lo;
-        // 1. histogram
-        constexpr int U = 8;   // loads in flight per thread
-        for (int64_t i0 = threadIdx.x; i0 < cnt; i0 += 256 * U) {
-            uint32_t k[U];
-#pragma unroll
-            for (int u = 0; u < U; u++) k[u] = i0 + u * 256 < cnt ? src_pairs[i0 + u * 256].x : 0u;
-#pragma unroll
-            for (int u = 0; u < U; u++)
-                if (i0 + u * 256 < cnt) atomicAdd(&s_h[phys((k[u] >> BKT_SHIFT) & bmask)], 1u);
-        }
+        // 1. histogram (the partition's pairs are the runs of the scatter's rounds)
+        constexpr int U = 16;   // loads in flight per thread: a tile of 32 runs (about 360 pairs at W = 22) in one round trip
+        part_walk_runs<U>(pairs, runs, p, n_chunks, [&](uint2 pr, bool v) {
+            if (v) atomicAdd(&s_h[phys((pr.x >> BKT_SHIFT) & bmask)], 1u);
+        });
         __syncthreads();
-        // 2. keep flags of the strip, the partition's survivor total and the strip's first slot
+        // 2. keep flags of the strip, the partition's survivor total and the strip's first slot.  Interior strips read the
+        // transposed histogram straight: bucket b0 + s * PER + j of the strip s = -1, 0, 1 is at (j << 8) + thread + s.
         uint32_t kept, S;
-        const uint64_t flags = pf_strip_flags(count, b0, PER, BP, rb, need, s_hl, s_hr, &kept);
+        const uint64_t flags = pf_strip_flags(count, [&](int s, int j) -> uint32_t { return s_h[(j << 8) + (int)threadIdx.x + s]; },
+                                              b0, PER, BP, rb, need, s_hl, s_hr, &kept);
         const uint32_t first = block_excl_scan_256(kept, s_warp, &S);
         if (threadIdx.x == 0) {
             lookback_publish(ts.status, gen, p, S);
@@ -572,7 +550,8 @@ __global__ void __launch_bounds__(256) k_part_filter(const uint2* __restrict__ p
             if (lane == 0) s_excl = ex;
         }
         // 3a. exclusive offsets of the kept buckets in place, their flag bits, the list of large buckets
-        pf_strip_offsets(count, b0, PER, flags, first, [&](int j, uint32_t off, bool f, uint32_t c) {
+        pf_strip_offsets([&](int b) -> uint32_t { return s_h[((b - b0) << 8) | threadIdx.x]; }, b0, PER, flags, first,
+                         [&](int j, uint32_t off, bool f, uint32_t c) {
             s_h[(j << 8) | threadIdx.x] = off;   // phys(b0 + j)
             const uint32_t bits = __ballot_sync(0xffffffffu, f);
             if (lane == 0) s_f[(j << 3) | warp] = bits;
@@ -588,16 +567,10 @@ __global__ void __launch_bounds__(256) k_part_filter(const uint2* __restrict__ p
         }
         uint2* st = spilled ? spill + s_excl : s_st;
         // 3b. survivors into their buckets' slot ranges (afterwards s_h[phys(b)] = end of bucket b)
-        for (int64_t i0 = threadIdx.x; i0 < cnt; i0 += 256 * U) {
-            uint2 pr[U];
-#pragma unroll
-            for (int u = 0; u < U; u++) pr[u] = i0 + u * 256 < cnt ? src_pairs[i0 + u * 256] : make_uint2(0u, 0u);
-#pragma unroll
-            for (int u = 0; u < U; u++) {
-                const uint32_t ph = phys((pr[u].x >> BKT_SHIFT) & bmask);
-                if (i0 + u * 256 < cnt && ((s_f[ph >> 5] >> (ph & 31)) & 1u)) st[atomicAdd(&s_h[ph], 1u)] = pr[u];
-            }
-        }
+        part_walk_runs<U>(pairs, runs, p, n_chunks, [&](uint2 pr, bool v) {
+            const uint32_t ph = phys((pr.x >> BKT_SHIFT) & bmask);
+            if (v && ((s_f[ph >> 5] >> (ph & 31)) & 1u)) st[atomicAdd(&s_h[ph], 1u)] = pr;
+        });
         __syncthreads();
         const uint32_t obase = s_excl;
         // 4a. small buckets: rank against the bucket, ties by slot
