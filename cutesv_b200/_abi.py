@@ -62,6 +62,10 @@ class csv_sa_cols(C.Structure):
                 ("mapq", _I32P), ("first_clip", _I32P), ("last_clip", _I32P), ("ref_span", _I32P)]
 
 
+class csv_seq_cols(C.Structure):
+    _fields_ = [("n_bytes", C.c_int64), ("seq_off", _I64P), ("seq4", _U8P)]
+
+
 CAND_DTYPE = np.dtype([
     ("svtype", "<i4"), ("chrom", "<i4"), ("pos", "<i4"), ("len", "<i4"), ("support", "<i4"),
     ("cipos", "<i4"), ("cilen", "<i4"), ("search_pos", "<i4"), ("pos2", "<i4"), ("aux", "<i4"),
@@ -156,7 +160,7 @@ def make_reads_cols(reads):
 SIG_FIELDS = ("chrom", "a", "b", "read_id", "c")
 READS_FIELDS = ("chrom", "start", "end", "read_id", "is_primary")
 _TYPESTR = {"is_primary": "|u1", "contig_off": "<i8"}   # every other column is int32 ("<i4")
-_ITEMSIZE = {"<i4": 4, "|u1": 1, "<i8": 8}
+_ITEMSIZE = {"<i4": 4, "|u1": 1, "<i8": 8, "<u4": 4, "<u1": 1}
 
 
 def is_device_array(x):
@@ -233,6 +237,78 @@ def device_cols(cols, fields, device, grouped=False, n_contigs=None):
     else:
         s = csv_reads_cols(n, *[C.cast(C.c_void_p(ptrs.get(f) if n else None), _U8P if f == "is_primary" else _I32P) for f in READS_FIELDS])
     return s, off
+
+
+READ_FIELDS = ("chrom", "ref_start", "ref_end", "flag", "mapq", "query_len", "read_id")
+SA_FIELDS = ("chrom", "pos0", "strand", "mapq", "first_clip", "last_clip", "ref_span")
+
+
+def _cai_check(name, v, typestrs, device):
+    """(address or None, length) of one device array; raises TypeError / ValueError like device_cols."""
+    cai = v.__cuda_array_interface__
+    if cai["typestr"] not in typestrs:
+        raise TypeError("column %s: dtype %s, expected %s" % (name, cai["typestr"], " or ".join(typestrs)))
+    shape = tuple(cai["shape"])
+    if len(shape) != 1:
+        raise TypeError("column %s: shape %s, expected one dimension" % (name, shape))
+    strides = cai.get("strides")
+    if strides is not None and shape[0] > 1 and tuple(strides) != (_ITEMSIZE[typestrs[0]],):
+        raise TypeError("column %s is not contiguous (strides %s)" % (name, tuple(strides)))
+    idx = _device_index(v)
+    if idx is not None and idx != device:
+        raise ValueError("column %s is on device %d, the engine on device %d" % (name, idx, device))
+    return (int(cai["data"][0]) if shape[0] else None), shape[0]
+
+
+
+def device_packet(packet, device):
+    """Normalises an alignment packet (the keys of packing.pack_alignments, plus optional seq_off / seq4: BAM's 4-bit packed bases)
+    whose arrays live in GPU memory.  Needs no GPU: it reads __cuda_array_interface__ and the arrays' device attribute only.
+
+    Returns None when every array is a host array (the numpy path of csv_extract).  Otherwise (csv_read_cols, cigar address,
+    n_cigar, csv_sa_cols, csv_seq_cols or None) of device addresses for csv_extract*_device.
+    Raises TypeError for an array of the wrong dtype (int32 record and SA columns, int64 offsets, uint32 or int32 CIGAR, uint8
+    bases), not 1-D or not contiguous; ValueError when host and device arrays are mixed, an array is on another device than
+    `device`, lengths disagree (n record columns, n + 1 offsets, equal SA columns), or only one of seq_off / seq4 is given.
+    Whether the addresses really are device memory of `device` is checked again by the library, the offsets' values on the device."""
+    sa = packet.get("sa") or {}
+    arrays = [(f, packet.get(f), ("<i4",)) for f in READ_FIELDS] + [(f, packet.get(f), ("<i8",)) for f in ("cigar_off", "sa_off")]
+    arrays += [("cigar", packet.get("cigar"), ("<u4", "<i4"))] + [("sa." + f, sa.get(f), ("<i4",)) for f in SA_FIELDS]
+    arrays += [("seq_off", packet.get("seq_off"), ("<i8",)), ("seq4", packet.get("seq4"), ("|u1", "<u1"))]
+    present = [(f, v, t) for f, v, t in arrays if v is not None]
+    on_dev = {f: is_device_array(v) for f, v, _ in present}
+    if not any(on_dev.values()):
+        return None
+    if not all(on_dev.values()):
+        raise ValueError("arrays of one packet must be all device or all host arrays: host %s, device %s"
+                         % (sorted(f for f, d in on_dev.items() if not d), sorted(f for f, d in on_dev.items() if d)))
+    missing = [f for f, v, _ in arrays[:len(READ_FIELDS) + 3 + len(SA_FIELDS)] if v is None]
+    if missing:
+        raise ValueError("packet arrays missing: %s" % missing)
+    if (packet.get("seq_off") is None) != (packet.get("seq4") is None):
+        raise ValueError("seq_off and seq4 go together: give both or neither")
+    ptrs, lens = {}, {}
+    for f, v, t in present:
+        ptrs[f], lens[f] = _cai_check(f, v, t, device)
+    n = lens["chrom"]
+    for f in READ_FIELDS:
+        if lens[f] != n:
+            raise ValueError("column lengths disagree: %s" % {g: lens[g] for g in READ_FIELDS})
+    for f in ("cigar_off", "sa_off") + (("seq_off",) if "seq_off" in lens else ()):
+        if lens[f] != n + 1:
+            raise ValueError("%s has %d entries, expected n + 1 = %d" % (f, lens[f], n + 1))
+    n_sa = lens["sa.chrom"]
+    if any(lens["sa." + f] != n_sa for f in SA_FIELDS):
+        raise ValueError("SA column lengths disagree: %s" % {f: lens["sa." + f] for f in SA_FIELDS})
+
+    def p(f, ctype=_I32P):
+        return C.cast(C.c_void_p(ptrs.get(f)), ctype)
+    reads = csv_read_cols(n, *[p(f) for f in READ_FIELDS], p("cigar_off", _I64P), p("sa_off", _I64P))
+    sa_cols = csv_sa_cols(n_sa, *[p("sa." + f) for f in SA_FIELDS])
+    seq = None
+    if "seq_off" in lens:
+        seq = csv_seq_cols(lens["seq4"], p("seq_off", _I64P), p("seq4", _U8P))
+    return reads, C.cast(C.c_void_p(ptrs["cigar"]), _U32P), lens["cigar"], sa_cols, seq
 
 
 def default_params(**kw):

@@ -225,17 +225,40 @@ class _Accumulator(object):
         return sorted_names
 
 
+def _tie_runs(chrom, a, b, read_id):
+    """INS rows sorted by (contig, int(pos), len, read, row) and the mask `same[k]`: sorted rows k and k + 1 tie on the first four.
+    None when there are fewer than two rows."""
+    n = len(chrom)
+    if n < 2:
+        return None
+    pos = np.asarray(a, dtype=np.int64) >> 1
+    order = np.lexsort((np.arange(n), read_id, b, pos, chrom))
+    k = np.stack([np.asarray(chrom)[order], pos[order], np.asarray(b)[order], np.asarray(read_id)[order]])
+    return order, np.all(k[:, 1:] == k[:, :-1], axis=0)
+
+
+def ins_tie_rows(chrom, a, b, read_id):
+    """Ascending INS rows that belong to a tie group of ins_tie_swaps (rows tying on (contig, int(pos), len, read)): the only rows
+    whose sequence strings ins_tie_swaps reads, so a caller whose strings live on the device fetches just these."""
+    runs = _tie_runs(chrom, a, b, read_id)
+    if runs is None:
+        return np.zeros(0, dtype=np.int64)
+    order, same = runs
+    member = np.zeros(len(order), dtype=bool)
+    member[1:] |= same
+    member[:-1] |= same
+    return np.sort(order[member]).astype(np.int64)
+
+
 def ins_tie_swaps(chrom, a, b, read_id, seqs):
     """Row swaps that put INS rows tying on (contig, int(pos), len, read) into the order of their sequence strings, the last
     field of the reference's INS sort key (cuteSV:774).  Vectorised search for tie groups (they need one read reporting two
     insertions of equal length at the same position: rare), selection sort inside a group.  Returns a list of (i, j)."""
-    n = len(chrom)
-    if n < 2:
+    runs = _tie_runs(chrom, a, b, read_id)
+    if runs is None:
         return []
-    pos = np.asarray(a, dtype=np.int64) >> 1
-    order = np.lexsort((np.arange(n), read_id, b, pos, chrom))
-    k = np.stack([np.asarray(chrom)[order], pos[order], np.asarray(b)[order], np.asarray(read_id)[order]])
-    same = np.all(k[:, 1:] == k[:, :-1], axis=0)
+    order, same = runs
+    n = len(order)
     if not same.any():
         return []
     pairs = []

@@ -105,6 +105,10 @@ struct ExtractState {
     uint32_t n_records = 0;          // alignment records of all packets of the accumulation (record index base of INS pieces)
     uint32_t n_skipped = 0;
     bool appending = false;
+    // INS sequence arena (csv_extract*_device with bases): ASCII bytes, start and length per INS row
+    DBuf ins_bytes, ins_start, ins_len, seq_tmp, seq_lb, seq_words, fetch_rows, fetch_off, fetch_out;
+    bool seq_valid = false;          // every packet of the accumulation carried bases
+    int64_t ins_nbytes = 0;
     double per_record[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // largest yield of a packet so far: signatures per type [0..4], pieces [5] per alignment record
 };
 
@@ -700,6 +704,7 @@ static int upload_sigs_impl(csv_ctx* c, int t, const csv_sig_cols* h, const int6
     s.has_c = h->c != nullptr;
     c->counts_valid = false;
     c->ex.rec_valid = false;
+    c->ex.seq_valid = false;
     c->up_checked[t] = false;
     if (h->n == 0) return CSV_OK;
     if ((!contig_off && !h->chrom) || !h->a || !h->b || !h->read_id) return set_err(CSV_E_INVALID, "null column");
@@ -743,6 +748,7 @@ static int upload_reads_impl(csv_ctx* c, const csv_reads_cols* h, const int64_t*
     c->n_reads = h->n;
     c->counts_valid = false;
     c->ex.rec_valid = false;
+    c->ex.seq_valid = false;
     c->up_checked[CSV_NTYPES] = false;
     if (h->n == 0) return CSV_OK;
     if ((!contig_off && !h->chrom) || !h->start || !h->end || !h->read_id || !h->is_primary) return set_err(CSV_E_INVALID, "null column");

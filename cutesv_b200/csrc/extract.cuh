@@ -239,4 +239,123 @@ __global__ void __launch_bounds__(EX_THREADS, EX_MIN_CTAS) k_extract(ReadView R,
     }
 }
 
+// ---- packets from device memory: offsets are checked on the device before any kernel reads through them ----
+enum { PK_BAD_CIGAR = 1u, PK_BAD_SA = 2u, PK_BAD_SEQ = 4u, PK_BAD_QLEN = 8u };
+struct PacketCheck {
+    const int64_t* off[3];   // cigar_off, sa_off, seq_off (n + 1 entries each; seq_off may be null)
+    int64_t bound[3];        // n_cigar, sa->n, seq->n_bytes
+    const int32_t* query_len;
+    int64_t n;
+};
+// *bad |= PK_BAD_* of every column whose offsets do not start at >= 0, never decrease and end at <= its bound, or that has a
+// negative query_len
+__global__ void __launch_bounds__(256) k_check_packet(PacketCheck C, uint32_t* bad) {
+    uint32_t b = 0;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= C.n; i += (int64_t)gridDim.x * blockDim.x) {
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+            const int64_t* o = C.off[k];
+            if (!o) continue;
+            const int64_t v = o[i];
+            if ((i == 0 && v < 0) || (i == C.n && v > C.bound[k]) || (i < C.n && o[i + 1] < v)) b |= 1u << k;
+        }
+        if (i < C.n && C.query_len[i] < 0) b |= PK_BAD_QLEN;
+    }
+    b = __reduce_or_sync(0xffffffffu, b);
+    if (b && (threadIdx.x & 31) == 0) atomicOr(bad, b);
+}
+
+// ---- INS sequences of one packet's new INS rows [first_row, first_row + m), built from the packed bases ----
+struct InsSeqJob {
+    const int32_t* piece_off; const int32_t* piece_cnt; const InsPiece* pieces;
+    int64_t first_row; int64_t m;
+    int32_t rec_base;                     // record index of the packet's first record (pieces hold global record indices)
+    const int64_t* seq_off; const uint8_t* seq4; const int32_t* query_len;
+    const uint32_t* cigar; const int64_t* cigar_off; const int32_t* ref_start;   // marker pieces: the record's CIGAR walk
+    int32_t min_siglength, merge_ins_threshold;
+};
+__device__ __forceinline__ SeqRec seq_rec(const InsSeqJob& J, int64_t rec) {
+    SeqRec s;
+    s.qlen = J.query_len[rec];
+    s.have = J.seq_off[rec + 1] - J.seq_off[rec] >= ((int64_t)s.qlen + 1) / 2;
+    s.seq4 = J.seq4 + J.seq_off[rec];
+    return s;
+}
+// arguments by value: a reference to the kernel parameter would give every thread of the common path a stack frame
+__device__ __noinline__ int64_t ins_marker(SeqRec s, const uint32_t* cigar, int64_t c0, int64_t c1, int32_t ref_start, int32_t pos,
+                                           int32_t min_siglength, int32_t merge_ins_threshold, uint8_t* out) {
+    return ins_marker_bytes(s, cigar + c0, c1 - c0, ref_start, pos, min_siglength, merge_ins_threshold, out);
+}
+__device__ __forceinline__ int64_t ins_marker(const InsSeqJob& J, const SeqRec& s, int64_t rec, int32_t pos, uint8_t* out) {
+    return ins_marker(s, J.cigar, J.cigar_off[rec], J.cigar_off[rec + 1], J.ref_start[rec], pos, J.min_siglength, J.merge_ins_threshold, out);
+}
+// len[k] = bytes of row first_row + k; *total64 += all of them (a 64-bit sum beside the 32-bit scan)
+__global__ void __launch_bounds__(256) k_ins_len(InsSeqJob J, uint32_t* len, unsigned long long* total64, uint32_t* status) {
+    for (int64_t base = (int64_t)blockIdx.x * blockDim.x; base < J.m; base += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t k = base + threadIdx.x;
+        int64_t w = 0;
+        if (k < J.m) {
+            const int64_t row = J.first_row + k;
+            const int32_t po = J.piece_off[row], pc = J.piece_cnt[row];
+            for (int32_t p = po; p < po + pc; p++) {
+                const InsPiece ip = J.pieces[p];
+                const int64_t rec = (int64_t)ip.rec - J.rec_base;
+                const SeqRec s = seq_rec(J, rec);
+                if (ip.rc == 2) {   // the length-only walk is inlined: a call here would make the loop spill across it
+                    const int64_t c0 = J.cigar_off[rec];
+                    const int64_t v = ins_marker_bytes(s, J.cigar + c0, J.cigar_off[rec + 1] - c0, J.ref_start[rec], ip.start, J.min_siglength,
+                                                       J.merge_ins_threshold, nullptr);
+                    if (v < 0) atomicOr(status, ST_INTERNAL);
+                    else w += v;
+                } else w += ins_piece_bytes(s, ip.start, ip.stop, ip.rc, nullptr, 0, 1);
+            }
+            len[k] = (uint32_t)w;
+        }
+        unsigned long long t = (unsigned long long)w;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+        if ((threadIdx.x & 31) == 0 && t) atomicAdd(total64, t);
+    }
+}
+// one warp per row: start[first_row + k] = arena_base + excl[k], the row's bytes at that offset
+__global__ void __launch_bounds__(256) k_ins_fill(InsSeqJob J, const uint32_t* excl, const uint32_t* len, int64_t arena_base, uint8_t* bytes,
+                                                  int64_t* start, int32_t* row_len) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+    for (int64_t k = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); k < J.m; k += warps) {
+        const int64_t row = J.first_row + k, o = arena_base + excl[k];
+        if (lane == 0) { start[row] = o; row_len[row] = (int32_t)len[k]; }
+        uint8_t* out = bytes + o;
+        const int32_t po = J.piece_off[row], pc = J.piece_cnt[row];
+        for (int32_t p = po; p < po + pc; p++) {
+            const InsPiece ip = J.pieces[p];
+            const int64_t rec = (int64_t)ip.rec - J.rec_base;
+            const SeqRec s = seq_rec(J, rec);
+            int64_t w;
+            if (ip.rc == 2) {   // rare: chains of more than MAX_OPEN_PIECES merged insertions, walked by one lane
+                int64_t v = 0;
+                if (lane == 0) v = ins_marker(J, s, rec, ip.start, out);
+                w = __shfl_sync(0xffffffffu, v, 0);
+                if (w < 0) w = 0;
+            } else w = ins_piece_bytes(s, ip.start, ip.stop, ip.rc, out, lane, 32);
+            out += w;
+        }
+    }
+}
+// csv_fetch_ins_seqs: one warp per requested row, out + off[i] <- the row's bytes
+__global__ void __launch_bounds__(256) k_ins_gather(const int64_t* rows, int64_t n, const int64_t* off, const uint8_t* bytes, const int64_t* start,
+                                                    const int32_t* row_len, uint8_t* out) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+    for (int64_t i = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); i < n; i += warps) {
+        const int64_t r = rows[i];
+        const uint8_t* src = bytes + start[r];
+        uint8_t* dst = out + off[i];
+        for (int32_t j = lane; j < row_len[r]; j += 32) dst[j] = src[j];
+    }
+}
+__global__ void k_ins_sel_len(const int64_t* rows, int64_t n, const int32_t* row_len, int32_t* len) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) len[i] = row_len[rows[i]];
+}
+
 }  // namespace csv

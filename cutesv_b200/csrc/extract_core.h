@@ -5,9 +5,10 @@
 // integer fields.  The CUDA kernel (extract.cuh) adds the warp-parallel CIGAR prefix scan; the
 // test-only emulator walks the CIGAR serially.  Citations "cuteSV:N" = src/cuteSV/cuteSV line N.
 //
-// INS sequences are never materialised on the device: every INS signature carries `seq_len` (what
-// clustering needs, resolveINDEL.py:400) and a list of "pieces" = Python slices of the record's
-// query sequence (or of its reverse complement) from which the host rebuilds the string.
+// Every INS signature carries `seq_len` (what clustering needs, resolveINDEL.py:400) and a list of
+// "pieces" = Python slices of the record's query sequence (or of its reverse complement) from which
+// the host rebuilds the string; for packets with bases in GPU memory the routines at the end of this
+// file build the same strings on the device.
 #pragma once
 #include "core.h"
 
@@ -371,5 +372,76 @@ CSV_HD void organize_split_signal(const SplitCtx& C, bool has_primary, const Seg
 
 // detect_flag (cuteSV:34-48): 1 forward primary (flag 0), 2 reverse primary (flag 16), else no SA analysis
 CSV_HD int detect_flag(int32_t flag) { return flag == 0 ? 1 : flag == 16 ? 2 : 0; }
+
+// ------------------------------------------------------------------------------------------
+// INS sequences built from BAM's 4-bit packed query (csv_extract_device with a csv_seq_cols): the same strings the host
+// builds from the piece list (cutesv_b200/packing.py ins_sequence / ins_block_from_packed), byte for byte.
+// ------------------------------------------------------------------------------------------
+// One record's packed bases: query_len bases from byte `seq4`, high nibble first.  have == false: BAM '*' (fewer than
+// (query_len + 1) / 2 bytes stored), every slice of it is empty.
+struct SeqRec { const uint8_t* seq4; int32_t qlen; bool have; };
+
+CSV_HD uint8_t seq_base(const SeqRec& s, int64_t j) {   // ASCII of query base j (0 <= j < qlen)
+    const uint8_t b = s.seq4[j >> 1];
+    return (uint8_t)"=ACMGRSVTWYHKDBN"[(j & 1) ? (b & 15) : (b >> 4)];
+}
+CSV_HD uint8_t seq_comp(uint8_t c) {   // packing._COMP: only ACGTN / acgtn are complemented, every other code is kept
+    switch (c) {
+        case 'A': return 'T'; case 'C': return 'G'; case 'G': return 'C'; case 'T': return 'A'; case 'N': return 'N';
+        case 'a': return 't'; case 'c': return 'g'; case 'g': return 'c'; case 't': return 'a'; case 'n': return 'n';
+        default: return c;
+    }
+}
+// Python slice [a:b] of a string of length L -> [lo, lo + len)
+CSV_HD void py_slice(int64_t a, int64_t b, int64_t L, int64_t* lo, int64_t* len) {
+    if (a < 0) { a += L; if (a < 0) a = 0; } else if (a > L) a = L;
+    if (b < 0) { b += L; if (b < 0) b = 0; } else if (b > L) b = L;
+    *lo = a;
+    *len = b > a ? b - a : 0;
+}
+// Bytes of piece (a, b, rc in {0, 1}): q[a:b], or revcomp(q)[a:b].  out == nullptr: length only.  Writes lanes
+// lane, lane + step, ... of the piece (step 1: all of it).
+CSV_HD int64_t ins_piece_bytes(const SeqRec& s, int32_t a, int32_t b, int32_t rc, uint8_t* out, int lane, int step) {
+    if (!s.have) return 0;
+    int64_t lo, len;
+    py_slice(a, b, s.qlen, &lo, &len);
+    if (out)
+        for (int64_t i = lane; i < len; i += step)
+            out[i] = rc ? seq_comp(seq_base(s, (int64_t)s.qlen - 1 - (lo + i))) : seq_base(s, lo + i);
+    return len;
+}
+// csv_fetch_ins_seqs: out_off[i] = start of the i-th requested row's string in the output (n + 1 entries), summed in 64 bits,
+// since the rows may repeat and span the whole accumulation.  Returns the total.
+CSV_HD int64_t ins_fetch_offsets(const int32_t* len, int64_t n, int64_t* out_off) {
+    int64_t o = 0;
+    for (int64_t i = 0; i < n; i++) { out_off[i] = o; o += len[i]; }
+    out_off[n] = o;
+    return o;
+}
+// Marker piece (rc == 2): the merged insertion that starts at reference position `pos`, rebuilt by the CIGAR walk of
+// packing.merged_ins_from_cigar (parse_read's walk, cuteSV:616-645, and generate_combine_sigs' INS chain, cuteSV:530-545).
+// Returns the string's length (out == nullptr: length only), -1 when no merged group starts at `pos`.
+CSV_HD int64_t ins_marker_bytes(const SeqRec& s, const uint32_t* cigar, int64_t n_ops, int32_t ref_start, int32_t pos,
+                                int32_t min_siglength, int32_t merge_ins_threshold, uint8_t* out) {
+    int64_t ref = ref_start;
+    int64_t q = (n_ops > 0 && (cigar[0] & 15) == OP_H) ? -(int64_t)(cigar[0] >> 4) : 0;   // shift_ins_read starts at -hardclip_left
+    bool open = false, target = false;
+    int64_t last = 0, written = 0;
+    for (int64_t k = 0; k < n_ops; k++) {
+        const int op = (int)(cigar[k] & 15);
+        const int64_t ln = (int64_t)(cigar[k] >> 4);
+        if (op != OP_D) q += ln;   // every op but D advances the query cursor (cuteSV:631-632)
+        if (ln >= min_siglength && (op == OP_I || op == OP_D)) {
+            if (op == OP_D) { ref += ln; continue; }
+            if (open && ref - last <= merge_ins_threshold) last = ref;   // joins the open group
+            else {
+                if (target) break;   // the group starting at pos is complete
+                open = true; last = ref; target = ref == pos;
+            }
+            if (target) written += ins_piece_bytes(s, (int32_t)(q - ln), (int32_t)q, 0, out ? out + written : nullptr, 0, 1);
+        } else if (op_ref_change(op)) ref += ln;
+    }
+    return target ? written : -1;
+}
 
 }  // namespace csv

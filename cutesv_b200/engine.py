@@ -400,10 +400,10 @@ class Engine(object):
 
 
 class _DeviceView(object):
-    """__cuda_array_interface__ of an int32 array the library owns (torch.as_tensor makes a view of it, no copy)."""
+    """__cuda_array_interface__ of an array the library owns (torch.as_tensor makes a view of it, no copy); int32 by default."""
 
-    def __init__(self, ptr, shape):
-        self.__cuda_array_interface__ = {"shape": tuple(shape), "typestr": "<i4", "data": (int(ptr or 0), False), "version": 2}
+    def __init__(self, ptr, shape, typestr="<i4"):
+        self.__cuda_array_interface__ = {"shape": tuple(shape), "typestr": typestr, "data": (int(ptr or 0), False), "version": 2}
 
 
 def _pin_packet_method(self, packed):
@@ -437,26 +437,38 @@ def _pin_packet_method(self, packed):
     return out
 
 
-def _extract_method(self, packed, append=False):
+def _extract_method(self, packed, append=False, stream=None):
     """csv_extract on a packing.pack_alignments() packet.  The extracted signatures and reads rows
     stay device-resident as the inputs of cluster_device(); returns dict(counts, n_rows).
     append=True (csv_extract_append): this packet's output is appended to what earlier packets left on the device;
-    counts / n_rows are the totals so far and `first` holds the totals before this packet."""
-    n = len(packed["chrom"])
-    keep = [np.ascontiguousarray(packed[k], dtype=np.int32) for k in ("chrom", "ref_start", "ref_end", "flag", "mapq", "query_len", "read_id")]
-    co = np.ascontiguousarray(packed["cigar_off"], dtype=np.int64)
-    so = np.ascontiguousarray(packed["sa_off"], dtype=np.int64)
-    rc_ = _abi.csv_read_cols(n, *[_abi.ptr(k) for k in keep], co.ctypes.data_as(C.POINTER(C.c_int64)), so.ctypes.data_as(C.POINTER(C.c_int64)))
-    sa = {k: np.ascontiguousarray(v, dtype=np.int32) for k, v in packed["sa"].items()}
-    sa_ = _abi.csv_sa_cols(len(sa["chrom"]), *[_abi.ptr(sa[k]) for k in ("chrom", "pos0", "strand", "mapq", "first_clip", "last_clip", "ref_span")])
-    cig = np.ascontiguousarray(packed["cigar"], dtype=np.uint32)
+    counts / n_rows are the totals so far and `first` holds the totals before this packet.
+    A packet whose arrays expose __cuda_array_interface__ (torch CUDA tensors; see _abi.device_packet) goes through
+    csv_extract*_device in the order of `stream` (see _producer_stream), and with seq_off / seq4 (BAM's packed bases) the INS
+    sequences are built on the device (fetch_ins_seqs, ins_seq_tensors).  Device and host packets may be mixed in one
+    append accumulation."""
     counts = (C.c_int64 * _abi.CSV_NTYPES)()
     n_rows = C.c_int64(0)
     first = list(getattr(self, "_ex_counts", [0] * _abi.CSV_NTYPES)) if (append and getattr(self, "_ex_appending", False)) else [0] * _abi.CSV_NTYPES
     first_rows = getattr(self, "_ex_rows", 0) if (append and getattr(self, "_ex_appending", False)) else 0
     first_pieces = getattr(self, "_ex_pieces", 0) if (append and getattr(self, "_ex_appending", False)) else 0
-    fn = self.L.csv_extract_append if append else self.L.csv_extract
-    _lib.check(fn(self.h, C.byref(rc_), cig.ctypes.data_as(C.POINTER(C.c_uint32)), C.c_int64(len(cig)), C.byref(sa_), counts, C.byref(n_rows)))
+    d = _abi.device_packet(packed, self.device)
+    if d is not None:
+        rc_, cig_p, n_cig, sa_, seq = d
+        st = self._producer_stream(stream, [packed])
+        fn = self.L.csv_extract_append_device if append else self.L.csv_extract_device
+        _lib.check(fn(self.h, C.byref(rc_), cig_p, C.c_int64(n_cig), C.byref(sa_), C.byref(seq) if seq is not None else None,
+                      C.c_void_p(st or None), counts, C.byref(n_rows)))
+    else:
+        n = len(packed["chrom"])
+        keep = [np.ascontiguousarray(packed[k], dtype=np.int32) for k in ("chrom", "ref_start", "ref_end", "flag", "mapq", "query_len", "read_id")]
+        co = np.ascontiguousarray(packed["cigar_off"], dtype=np.int64)
+        so = np.ascontiguousarray(packed["sa_off"], dtype=np.int64)
+        rc_ = _abi.csv_read_cols(n, *[_abi.ptr(k) for k in keep], co.ctypes.data_as(C.POINTER(C.c_int64)), so.ctypes.data_as(C.POINTER(C.c_int64)))
+        sa = {k: np.ascontiguousarray(v, dtype=np.int32) for k, v in packed["sa"].items()}
+        sa_ = _abi.csv_sa_cols(len(sa["chrom"]), *[_abi.ptr(sa[k]) for k in ("chrom", "pos0", "strand", "mapq", "first_clip", "last_clip", "ref_span")])
+        cig = np.ascontiguousarray(packed["cigar"], dtype=np.uint32)
+        fn = self.L.csv_extract_append if append else self.L.csv_extract
+        _lib.check(fn(self.h, C.byref(rc_), cig.ctypes.data_as(C.POINTER(C.c_uint32)), C.c_int64(len(cig)), C.byref(sa_), counts, C.byref(n_rows)))
     self._ex_counts = [int(x) for x in counts]
     self._ex_rows = int(n_rows.value)
     self._dev_rows = self._ex_counts + [self._ex_rows]
@@ -467,6 +479,41 @@ def _extract_method(self, packed, append=False):
     return dict(counts={name: int(counts[t]) for t, name in enumerate(_abi.TYPE_NAMES)}, n_rows=int(n_rows.value),
                 first={name: first[t] for t, name in enumerate(_abi.TYPE_NAMES)}, first_rows=first_rows, first_pieces=first_pieces,
                 n_pieces=self._ex_pieces)
+
+
+def _fetch_ins_seqs_method(self, rows):
+    """Sequence strings of INS rows `rows` from the device-built arena (csv_fetch_ins_seqs: one gather, one D2H copy).
+    Needs an accumulation whose packets all were device packets with bases; CuteSVError CSV_E_STATE otherwise."""
+    rows = np.ascontiguousarray(rows, dtype=np.int64).reshape(-1)
+    n = len(rows)
+    off = np.zeros(n + 1, dtype=np.int64)
+    cap = 512 * n + 4096
+    while True:
+        out = np.zeros(max(cap, 1), dtype=np.uint8)
+        rc = self.L.csv_fetch_ins_seqs(self.h, rows.ctypes.data_as(C.POINTER(C.c_int64)), C.c_int64(n), out.ctypes.data_as(C.POINTER(C.c_uint8)),
+                                       C.c_int64(cap), off.ctypes.data_as(C.POINTER(C.c_int64)))
+        if rc != _abi.CSV_E_CAPACITY:
+            break
+        cap = int(off[n])
+    _lib.check(rc)
+    whole = out[:int(off[n])].tobytes().decode("ascii")
+    o = off.tolist()
+    return [whole[o[i]:o[i + 1]] for i in range(n)]
+
+
+def _ins_seq_tensors_method(self):
+    """Zero-copy torch views of the device-built INS sequence arena: (bytes uint8, start int64 [n_rows], length int32 [n_rows]);
+    row k's string is bytes[start[k]:start[k] + length[k]].  Valid until the next extract, upload or swap_ins_rows on this
+    engine, so clone() whatever you keep."""
+    import torch
+    b, s, ln, nr = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_int64(0)
+    _lib.check(self.L.csv_ins_seq_device_ptrs(self.h, C.byref(b), C.byref(s), C.byref(ln), C.byref(nr)))
+    dev = torch.device("cuda", self.device)
+    n = nr.value
+    start = torch.as_tensor(_DeviceView(s.value, (n,), "<i8"), device=dev)
+    length = torch.as_tensor(_DeviceView(ln.value, (n,)), device=dev)
+    nbytes = int((start + length.to(torch.int64)).max()) if n else 0
+    return torch.as_tensor(_DeviceView(b.value, (nbytes,), "|u1"), device=dev), start, length
 
 
 def _extract_skipped_method(self):
@@ -568,4 +615,6 @@ Engine.remap_read_ids = _remap_read_ids_method
 Engine.fetch_read_rows = _fetch_read_rows_method
 Engine.swap_ins_rows = _swap_ins_rows_method
 Engine.extract = _extract_method
+Engine.fetch_ins_seqs = _fetch_ins_seqs_method
+Engine.ins_seq_tensors = _ins_seq_tensors_method
 Engine.fetch_extracted = _fetch_extracted_method

@@ -72,6 +72,29 @@ def pack_alignments(reads, chrom_id, read_id):
 
 
 _COMP = str.maketrans("ACGTNacgtn", "TGCANtgcan")
+_NIB_CODE = np.full(256, 15, dtype=np.uint8)   # BAM's 4-bit base codes, "=ACMGRSVTWYHKDBN"; any other character packs as N
+for _i, _ch in enumerate("=ACMGRSVTWYHKDBN"):
+    _NIB_CODE[ord(_ch)] = _i
+    _NIB_CODE[ord(_ch.lower())] = _i
+
+
+def pack_bases(strings):
+    """BAM's 4-bit packed form of query sequences (high nibble first, "=ACMGRSVTWYHKDBN"; lower case packs as upper case):
+    returns (seq4 uint8, seq_off int64 [n + 1]), the layout of bamio.BamReader.next_packet.  None or "" stores no bases
+    (BAM '*')."""
+    lens = np.fromiter((len(s) if s else 0 for s in strings), dtype=np.int64, count=len(strings))
+    nb = (lens + 1) // 2
+    seq_off = np.zeros(len(strings) + 1, dtype=np.int64)
+    np.cumsum(nb, out=seq_off[1:])
+    seq4 = np.zeros(int(seq_off[-1]), dtype=np.uint8)
+    for i, s in enumerate(strings):
+        if not s:
+            continue
+        code = _NIB_CODE[np.frombuffer(s.encode("ascii"), dtype=np.uint8)]
+        if len(code) & 1:
+            code = np.append(code, np.uint8(0))
+        seq4[seq_off[i]:seq_off[i + 1]] = (code[0::2] << 4) | code[1::2]
+    return seq4, seq_off
 
 
 def revcomp(s):

@@ -355,6 +355,49 @@ int csv_extract(csv_ctx* ctx, const csv_read_cols* reads, const uint32_t* cigar,
 int csv_extract_append(csv_ctx* ctx, const csv_read_cols* reads, const uint32_t* cigar, int64_t n_cigar,
                        const csv_sa_cols* sa, int64_t counts[CSV_NTYPES], int64_t* n_read_rows);
 int csv_extract_reset(csv_ctx* ctx);
+
+/* ---- extraction from alignment records that already live in GPU memory (a GPU aligner, a PyTorch pipeline) ----
+ * Query bases in BAM's 4-bit packed form ("=ACMGRSVTWYHKDBN", high nibble first): record i's bases start at byte
+ * seq_off[i] (n + 1 entries), query_len[i] bases are expected.  A record with fewer than (query_len + 1) / 2 stored bytes has
+ * no stored sequence (BAM '*'): its INS slices are empty.  bamio.BamReader.next_packet produces this layout. */
+typedef struct csv_seq_cols {
+    int64_t n_bytes;
+    const int64_t* seq_off;
+    const uint8_t* seq4;
+} csv_seq_cols;
+/* csv_extract / csv_extract_append (same results, counters, record column and skipped-record count) on a packet whose
+ * columns, CIGAR stream, SA table and bases (seq, may be NULL) are device or managed memory on the ctx's device, as
+ * cudaPointerGetAttributes reports it; anything else is CSV_E_INVALID naming the column.  Device and host packets may be
+ * mixed in one append accumulation.
+ *   - Stream order both ways: the call's device work waits for everything enqueued on `stream` (NULL = the legacy default
+ *     stream) before it, and `stream` waits for the call's last read of the caller's memory.  The call blocks the host
+ *     until the output counts are known, as the host calls do.
+ *   - Only the CIGAR stream is copied (into the ctx's padded buffer: the kernel's bulk copies read whole tiles); the other
+ *     columns and the bases are read in place during the call.
+ *   - The offsets are checked on the device before any kernel reads through them: cigar_off, sa_off and seq_off must start
+ *     at >= 0, never decrease and end at <= n_cigar, sa->n and seq->n_bytes; query_len must be >= 0.  A failure is
+ *     CSV_E_INPUT naming the column and changes nothing: the previous accumulation and its counters stay as they were.
+ *   - With seq, the sequence of every new INS signature is built on the device into a ctx-owned arena, appended per packet:
+ *     row k's string is bytes[start[k] .. start[k] + len[k]), byte-identical to what the host builds from the piece list
+ *     (cutesv_b200/packing.py ins_sequence, marker pieces included).  The arena is valid while every packet of the
+ *     accumulation carried seq; any other extraction, csv_extract_reset or a signature / reads upload invalidates it.
+ *     csv_swap_ins_rows keeps it attached to the rows, csv_remap_read_ids leaves it alone.  The strings of one packet must
+ *     stay below 4 GiB, else CSV_E_CAPACITY: an append call then leaves the accumulation as it was, a non-append call leaves
+ *     it empty (as csv_extract_reset does; its kernel has already overwritten the previous rows). */
+int csv_extract_device(csv_ctx* ctx, const csv_read_cols* reads, const uint32_t* cigar, int64_t n_cigar, const csv_sa_cols* sa,
+                       const csv_seq_cols* seq, void* stream, int64_t counts[CSV_NTYPES], int64_t* n_read_rows);
+int csv_extract_append_device(csv_ctx* ctx, const csv_read_cols* reads, const uint32_t* cigar, int64_t n_cigar, const csv_sa_cols* sa,
+                              const csv_seq_cols* seq, void* stream, int64_t counts[CSV_NTYPES], int64_t* n_read_rows);
+/* Device pointers of the INS sequence arena, for a caller's own CUDA code: ASCII bases, the int64 start and the int32 length
+ * of every INS row (n_rows = the INS signature count).  Blocks until the arena is complete.  Valid until the next
+ * extraction, upload, csv_swap_ins_rows or csv_destroy.  CSV_E_STATE when the arena is not valid. */
+int csv_ins_seq_device_ptrs(csv_ctx* ctx, const uint8_t** bytes, const int64_t** start, const int32_t** len, int64_t* n_rows);
+/* Strings of INS rows rows[0..n) (any order, repeats allowed) gathered on the device, one D2H copy of the strings: row rows[i]
+ * is out[out_off[i] .. out_off[i + 1]) (out_off: n + 1 entries, 64-bit, so the total may exceed 4 GiB).  On CSV_E_CAPACITY
+ * out_off is filled and out_off[n] is the size `out` needs.  CSV_E_STATE when the arena is not valid, CSV_E_INVALID for a row
+ * outside the INS signatures. */
+int csv_fetch_ins_seqs(csv_ctx* ctx, const int64_t* rows, int64_t n, uint8_t* out, int64_t cap, int64_t* out_off);
+
 /* Records whose split-read analysis was skipped because they carry more than 64 qualifying segments (only reachable
  * with --max_split_parts -1; their CIGAR signatures are taken).  The reference has no such limit: a documented,
  * counted deviation instead of a failed run. */
@@ -362,7 +405,8 @@ int64_t csv_extract_skipped(csv_ctx* ctx);
 /* read_id of every device-resident signature / reads-table row: id -> rank[id].  The CLI numbers read names in
  * first-seen order while it decodes and learns their ranks in Python string order at the end (cuteSV:764-801). */
 int csv_remap_read_ids(csv_ctx* ctx, const int32_t* rank, int64_t n_rank);
-/* Swap rows pairs[2k] <-> pairs[2k+1] of the device-resident INS signatures (columns and piece descriptors), in
+/* Swap rows pairs[2k] <-> pairs[2k+1] of the device-resident INS signatures (columns, piece descriptors and, while it is
+ * valid, the sequence arena's start and length), in
  * sequence.  INS rows that tie on (contig, int(pos), len, read) must be in the order of their sequence strings
  * (the reference's sort key ends with the sequence, cuteSV:774); the host, which owns the strings, fixes the few
  * ties of device-extracted rows with this call. */
