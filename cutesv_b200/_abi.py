@@ -66,6 +66,10 @@ class csv_seq_cols(C.Structure):
     _fields_ = [("n_bytes", C.c_int64), ("seq_off", _I64P), ("seq4", _U8P)]
 
 
+class csv_name_cols(C.Structure):
+    _fields_ = [("n_bytes", C.c_int64), ("name_off", _I64P), ("names", _U8P)]
+
+
 CAND_DTYPE = np.dtype([
     ("svtype", "<i4"), ("chrom", "<i4"), ("pos", "<i4"), ("len", "<i4"), ("support", "<i4"),
     ("cipos", "<i4"), ("cilen", "<i4"), ("search_pos", "<i4"), ("pos2", "<i4"), ("aux", "<i4"),
@@ -261,40 +265,58 @@ def _cai_check(name, v, typestrs, device):
 
 
 
-def device_packet(packet, device):
-    """Normalises an alignment packet (the keys of packing.pack_alignments, plus optional seq_off / seq4: BAM's 4-bit packed bases)
-    whose arrays live in GPU memory.  Needs no GPU: it reads __cuda_array_interface__ and the arrays' device attribute only.
+class DevicePacket(tuple):
+    """device_packet's result: unpacks as (csv_read_cols, cigar address, n_cigar, csv_sa_cols, csv_seq_cols or None); `names` is
+    the csv_name_cols of a named packet (csv_extract*_named_device), else None."""
+    names = None
 
-    Returns None when every array is a host array (the numpy path of csv_extract).  Otherwise (csv_read_cols, cigar address,
-    n_cigar, csv_sa_cols, csv_seq_cols or None) of device addresses for csv_extract*_device.
+
+def device_packet(packet, device):
+    """Normalises an alignment packet (the keys of packing.pack_alignments, plus optional seq_off / seq4: BAM's 4-bit packed bases,
+    and optional names / name_off: the records' read names as bytes) whose arrays live in GPU memory.  Needs no GPU: it reads
+    __cuda_array_interface__ and the arrays' device attribute only.
+
+    Returns None when every array is a host array (the numpy path of csv_extract).  Otherwise a DevicePacket: (csv_read_cols,
+    cigar address, n_cigar, csv_sa_cols, csv_seq_cols or None) of device addresses for csv_extract*_device, with `.names` the
+    csv_name_cols of a named packet (record i's name is names[name_off[i]:name_off[i + 1]]; such a packet has no read_id).
     Raises TypeError for an array of the wrong dtype (int32 record and SA columns, int64 offsets, uint32 or int32 CIGAR, uint8
-    bases), not 1-D or not contiguous; ValueError when host and device arrays are mixed, an array is on another device than
-    `device`, lengths disagree (n record columns, n + 1 offsets, equal SA columns), or only one of seq_off / seq4 is given.
+    bases and names), not 1-D or not contiguous; ValueError when host and device arrays are mixed (names on a host packet
+    included), an array is on another device than `device`, lengths disagree (n record columns, n + 1 offsets, equal SA
+    columns), only one of seq_off / seq4 or of names / name_off is given, or read_id comes with names.
     Whether the addresses really are device memory of `device` is checked again by the library, the offsets' values on the device."""
     sa = packet.get("sa") or {}
+    named = packet.get("names") is not None or packet.get("name_off") is not None
     arrays = [(f, packet.get(f), ("<i4",)) for f in READ_FIELDS] + [(f, packet.get(f), ("<i8",)) for f in ("cigar_off", "sa_off")]
     arrays += [("cigar", packet.get("cigar"), ("<u4", "<i4"))] + [("sa." + f, sa.get(f), ("<i4",)) for f in SA_FIELDS]
     arrays += [("seq_off", packet.get("seq_off"), ("<i8",)), ("seq4", packet.get("seq4"), ("|u1", "<u1"))]
+    arrays += [("name_off", packet.get("name_off"), ("<i8",)), ("names", packet.get("names"), ("|u1", "<u1"))]
     present = [(f, v, t) for f, v, t in arrays if v is not None]
     on_dev = {f: is_device_array(v) for f, v, _ in present}
     if not any(on_dev.values()):
+        if named:
+            raise ValueError("names / name_off are accepted on device packets only (a host packet carries read_id)")
         return None
     if not all(on_dev.values()):
         raise ValueError("arrays of one packet must be all device or all host arrays: host %s, device %s"
                          % (sorted(f for f, d in on_dev.items() if not d), sorted(f for f, d in on_dev.items() if d)))
-    missing = [f for f, v, _ in arrays[:len(READ_FIELDS) + 3 + len(SA_FIELDS)] if v is None]
+    if named and packet.get("read_id") is not None:
+        raise ValueError("a named packet carries no read_id: the library numbers its records and ranks their names")
+    missing = [f for f, v, _ in arrays[:len(READ_FIELDS) + 3 + len(SA_FIELDS)] if v is None and not (named and f == "read_id")]
     if missing:
         raise ValueError("packet arrays missing: %s" % missing)
     if (packet.get("seq_off") is None) != (packet.get("seq4") is None):
         raise ValueError("seq_off and seq4 go together: give both or neither")
+    if (packet.get("name_off") is None) != (packet.get("names") is None):
+        raise ValueError("name_off and names go together: give both or neither")
     ptrs, lens = {}, {}
     for f, v, t in present:
         ptrs[f], lens[f] = _cai_check(f, v, t, device)
     n = lens["chrom"]
-    for f in READ_FIELDS:
+    rfields = [f for f in READ_FIELDS if f in lens]
+    for f in rfields:
         if lens[f] != n:
-            raise ValueError("column lengths disagree: %s" % {g: lens[g] for g in READ_FIELDS})
-    for f in ("cigar_off", "sa_off") + (("seq_off",) if "seq_off" in lens else ()):
+            raise ValueError("column lengths disagree: %s" % {g: lens[g] for g in rfields})
+    for f in ("cigar_off", "sa_off") + tuple(f for f in ("seq_off", "name_off") if f in lens):
         if lens[f] != n + 1:
             raise ValueError("%s has %d entries, expected n + 1 = %d" % (f, lens[f], n + 1))
     n_sa = lens["sa.chrom"]
@@ -308,7 +330,10 @@ def device_packet(packet, device):
     seq = None
     if "seq_off" in lens:
         seq = csv_seq_cols(lens["seq4"], p("seq_off", _I64P), p("seq4", _U8P))
-    return reads, C.cast(C.c_void_p(ptrs["cigar"]), _U32P), lens["cigar"], sa_cols, seq
+    out = DevicePacket((reads, C.cast(C.c_void_p(ptrs["cigar"]), _U32P), lens["cigar"], sa_cols, seq))
+    if named:
+        out.names = csv_name_cols(lens["names"], p("name_off", _I64P), p("names", _U8P))
+    return out
 
 
 def default_params(**kw):

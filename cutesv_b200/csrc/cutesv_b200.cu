@@ -109,6 +109,13 @@ struct ExtractState {
     DBuf ins_bytes, ins_start, ins_len, seq_tmp, seq_lb, seq_words, fetch_rows, fetch_off, fetch_out;
     bool seq_valid = false;          // every packet of the accumulation carried bases
     int64_t ins_nbytes = 0;
+    // read-name arena (csv_extract*_named_device): the names of all records of the accumulation, name i at bytes
+    // [name_off[i], name_off[i + 1]); the records' provisional read ids are their indices.  csv_rank_names adds the tables
+    // record -> dense rank and rank -> (start, length).
+    DBuf name_bytes, name_off, pid, name_rank, name_tab_start, name_tab_len, name_words;
+    bool named = false;              // every packet of the accumulation carried names
+    bool ranked = false;             // csv_rank_names has turned the provisional ids into ranks
+    int64_t name_nbytes = 0, n_names = 0;
     double per_record[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // largest yield of a packet so far: signatures per type [0..4], pieces [5] per alignment record
 };
 
@@ -705,6 +712,7 @@ static int upload_sigs_impl(csv_ctx* c, int t, const csv_sig_cols* h, const int6
     c->counts_valid = false;
     c->ex.rec_valid = false;
     c->ex.seq_valid = false;
+    c->ex.named = false; c->ex.ranked = false;   // the rows no longer come from the named accumulation
     c->up_checked[t] = false;
     if (h->n == 0) return CSV_OK;
     if ((!contig_off && !h->chrom) || !h->a || !h->b || !h->read_id) return set_err(CSV_E_INVALID, "null column");
@@ -749,6 +757,7 @@ static int upload_reads_impl(csv_ctx* c, const csv_reads_cols* h, const int64_t*
     c->counts_valid = false;
     c->ex.rec_valid = false;
     c->ex.seq_valid = false;
+    c->ex.named = false; c->ex.ranked = false;   // the rows no longer come from the named accumulation
     c->up_checked[CSV_NTYPES] = false;
     if (h->n == 0) return CSV_OK;
     if ((!contig_off && !h->chrom) || !h->start || !h->end || !h->read_id || !h->is_primary) return set_err(CSV_E_INVALID, "null column");
@@ -1695,3 +1704,4 @@ extern "C" int csv_sort_probe(csv_ctx* c, float* ms_total, int64_t* bytes_total,
 #include "gather_api.inl"
 #include "genotype_api.inl"
 #include "sigsort_api.inl"
+#include "names_api.inl"

@@ -4,6 +4,7 @@
 // engine (cuteSV:50-513).  HBM-bound: 4 B per CIGAR op read once, coalesced.
 #pragma once
 #include "extract_core.h"
+#include "names_core.h"
 
 namespace csv {
 
@@ -240,24 +241,26 @@ __global__ void __launch_bounds__(EX_THREADS, EX_MIN_CTAS) k_extract(ReadView R,
 }
 
 // ---- packets from device memory: offsets are checked on the device before any kernel reads through them ----
-enum { PK_BAD_CIGAR = 1u, PK_BAD_SA = 2u, PK_BAD_SEQ = 4u, PK_BAD_QLEN = 8u };
+enum { PK_BAD_CIGAR = 1u, PK_BAD_SA = 2u, PK_BAD_SEQ = 4u, PK_BAD_QLEN = 8u, PK_BAD_NAME = 16u, PK_LONG_NAME = 32u };
 struct PacketCheck {
-    const int64_t* off[3];   // cigar_off, sa_off, seq_off (n + 1 entries each; seq_off may be null)
-    int64_t bound[3];        // n_cigar, sa->n, seq->n_bytes
+    const int64_t* off[4];   // cigar_off, sa_off, seq_off, name_off (n + 1 entries each; seq_off and name_off may be null)
+    int64_t bound[4];        // n_cigar, sa->n, seq->n_bytes, names->n_bytes
     const int32_t* query_len;
     int64_t n;
 };
 // *bad |= PK_BAD_* of every column whose offsets do not start at >= 0, never decrease and end at <= its bound, or that has a
-// negative query_len
+// negative query_len; PK_LONG_NAME for a name longer than NAME_MAX_BYTES
 __global__ void __launch_bounds__(256) k_check_packet(PacketCheck C, uint32_t* bad) {
     uint32_t b = 0;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= C.n; i += (int64_t)gridDim.x * blockDim.x) {
 #pragma unroll
-        for (int k = 0; k < 3; k++) {
+        for (int k = 0; k < 4; k++) {
             const int64_t* o = C.off[k];
             if (!o) continue;
             const int64_t v = o[i];
-            if ((i == 0 && v < 0) || (i == C.n && v > C.bound[k]) || (i < C.n && o[i + 1] < v)) b |= 1u << k;
+            const uint32_t bit = k < 3 ? 1u << k : PK_BAD_NAME;
+            if ((i == 0 && v < 0) || (i == C.n && v > C.bound[k]) || (i < C.n && o[i + 1] < v)) b |= bit;
+            if (k == 3 && i < C.n && o[i + 1] - v > NAME_MAX_BYTES) b |= PK_LONG_NAME;
         }
         if (i < C.n && C.query_len[i] < 0) b |= PK_BAD_QLEN;
     }

@@ -445,7 +445,9 @@ def _extract_method(self, packed, append=False, stream=None):
     A packet whose arrays expose __cuda_array_interface__ (torch CUDA tensors; see _abi.device_packet) goes through
     csv_extract*_device in the order of `stream` (see _producer_stream), and with seq_off / seq4 (BAM's packed bases) the INS
     sequences are built on the device (fetch_ins_seqs, ins_seq_tensors).  Device and host packets may be mixed in one
-    append accumulation."""
+    append accumulation.  A device packet with names / name_off (the records' read names as bytes, instead of read_id) goes
+    through csv_extract*_named_device: every packet of the accumulation then carries names, and rank_names() turns the
+    provisional ids (record indices) into name ranks."""
     counts = (C.c_int64 * _abi.CSV_NTYPES)()
     n_rows = C.c_int64(0)
     first = list(getattr(self, "_ex_counts", [0] * _abi.CSV_NTYPES)) if (append and getattr(self, "_ex_appending", False)) else [0] * _abi.CSV_NTYPES
@@ -455,9 +457,14 @@ def _extract_method(self, packed, append=False, stream=None):
     if d is not None:
         rc_, cig_p, n_cig, sa_, seq = d
         st = self._producer_stream(stream, [packed])
-        fn = self.L.csv_extract_append_device if append else self.L.csv_extract_device
-        _lib.check(fn(self.h, C.byref(rc_), cig_p, C.c_int64(n_cig), C.byref(sa_), C.byref(seq) if seq is not None else None,
-                      C.c_void_p(st or None), counts, C.byref(n_rows)))
+        seq_p = C.byref(seq) if seq is not None else None
+        if d.names is not None:
+            fn = self.L.csv_extract_append_named_device if append else self.L.csv_extract_named_device
+            _lib.check(fn(self.h, C.byref(rc_), cig_p, C.c_int64(n_cig), C.byref(sa_), seq_p, C.byref(d.names), C.c_void_p(st or None), counts,
+                          C.byref(n_rows)))
+        else:
+            fn = self.L.csv_extract_append_device if append else self.L.csv_extract_device
+            _lib.check(fn(self.h, C.byref(rc_), cig_p, C.c_int64(n_cig), C.byref(sa_), seq_p, C.c_void_p(st or None), counts, C.byref(n_rows)))
     else:
         n = len(packed["chrom"])
         keep = [np.ascontiguousarray(packed[k], dtype=np.int32) for k in ("chrom", "ref_start", "ref_end", "flag", "mapq", "query_len", "read_id")]
@@ -514,6 +521,52 @@ def _ins_seq_tensors_method(self):
     length = torch.as_tensor(_DeviceView(ln.value, (n,)), device=dev)
     nbytes = int((start + length.to(torch.int64)).max()) if n else 0
     return torch.as_tensor(_DeviceView(b.value, (nbytes,), "|u1"), device=dev), start, length
+
+
+def _rank_names_method(self):
+    """Ranks the read names of a named accumulation on the device (csv_rank_names): every signature's and reads row's read id
+    becomes the dense rank of its name in byte (for UTF-8: Python str) order.  Returns the number of distinct names."""
+    nd = C.c_int64(0)
+    _lib.check(self.L.csv_rank_names(self.h, C.byref(nd)))
+    return int(nd.value)
+
+
+def _fetch_names_method(self, ranks):
+    """Read names (str) of name ranks `ranks` (any order, repeats allowed) after rank_names (csv_fetch_names)."""
+    ranks = np.ascontiguousarray(ranks, dtype=np.int32).reshape(-1)
+    n = len(ranks)
+    off = np.zeros(n + 1, dtype=np.int64)
+    cap = 64 * n + 256
+    while True:
+        out = np.zeros(max(cap, 1), dtype=np.uint8)
+        rc = self.L.csv_fetch_names(self.h, _abi.ptr(ranks), C.c_int64(n), out.ctypes.data_as(C.POINTER(C.c_uint8)), C.c_int64(cap),
+                                    off.ctypes.data_as(C.POINTER(C.c_int64)))
+        if rc != _abi.CSV_E_CAPACITY:
+            break
+        cap = int(off[n])
+    _lib.check(rc)
+    raw = out[:int(off[n])].tobytes()
+    o = off.tolist()
+    return [raw[o[i]:o[i + 1]].decode("utf-8") for i in range(n)]
+
+
+def _name_rank_tensor_method(self):
+    """Zero-copy torch view (int32, one entry per record of the accumulation) of the table record index -> name rank that
+    rank_names built, e.g. to turn a caller-built alignment table's provisional ids into ranks with one gather.  Valid until the
+    next extract or extract_reset on this engine, so clone() what you keep."""
+    import torch
+    p, nr = C.c_void_p(), C.c_int64(0)
+    _lib.check(self.L.csv_name_ranks_device_ptr(self.h, C.byref(p), C.byref(nr)))
+    return torch.as_tensor(_DeviceView(p.value, (nr.value,)), device=torch.device("cuda", self.device))
+
+
+def _order_ins_ties_method(self):
+    """Puts INS rows that tie on (contig, int(pos), len, read) into the order of their device-built sequences (csv_order_ins_ties):
+    what ins_tie_swaps + swap_ins_rows do on the host.  The read ids must be ranks (rank_names or remap_read_ids first).  Returns
+    the number of rows whose content moved."""
+    nm = C.c_int64(0)
+    _lib.check(self.L.csv_order_ins_ties(self.h, C.byref(nm)))
+    return int(nm.value)
 
 
 def _extract_skipped_method(self):
@@ -618,3 +671,7 @@ Engine.extract = _extract_method
 Engine.fetch_ins_seqs = _fetch_ins_seqs_method
 Engine.ins_seq_tensors = _ins_seq_tensors_method
 Engine.fetch_extracted = _fetch_extracted_method
+Engine.rank_names = _rank_names_method
+Engine.fetch_names = _fetch_names_method
+Engine.name_rank_tensor = _name_rank_tensor_method
+Engine.order_ins_ties = _order_ins_ties_method

@@ -398,6 +398,55 @@ int csv_ins_seq_device_ptrs(csv_ctx* ctx, const uint8_t** bytes, const int64_t**
  * outside the INS signatures. */
 int csv_fetch_ins_seqs(csv_ctx* ctx, const int64_t* rows, int64_t n, uint8_t* out, int64_t cap, int64_t* out_off);
 
+/* ---- read names of device packets, ranked on the device ----
+ * The reference's sort keys break ties on the read name in Python string order (cuteSV:764-801), so every read id must be
+ * the rank of its name across the whole run.  A named packet carries the names instead of ids: record i's name is
+ * names[name_off[i] .. name_off[i + 1]) (name_off: n + 1 entries), without a NUL terminator, compared as bytes (for UTF-8
+ * text byte order is Python str order). */
+typedef struct csv_name_cols {
+    int64_t n_bytes;
+    const int64_t* name_off;
+    const uint8_t* names;
+} csv_name_cols;
+/* csv_extract_device / csv_extract_append_device on a named packet (device memory, like every other column); reads->read_id
+ * must be NULL (CSV_E_INVALID otherwise).
+ *   - Each record gets a provisional read id: its index in the accumulation (the records of earlier packets plus the
+ *     packet-local index, the numbering of csv_fetch_records).  csv_rank_names turns these into ranks.
+ *   - The names are copied device to device into a ctx-owned arena, appended per packet, in the stream order of the CIGAR copy.
+ *   - name_off is checked on the device with the other offsets: start >= 0, never decreasing, end <= n_bytes, every name at
+ *     most 254 bytes (BAM's limit).  A failure is CSV_E_INPUT naming the column and changes nothing.
+ *   - CSV_E_STATE, changing nothing: a named packet appended to an accumulation of unnamed packets or the reverse (host
+ *     packets included), or any append after csv_rank_names (csv_extract_reset or a fresh extraction starts over). */
+int csv_extract_named_device(csv_ctx* ctx, const csv_read_cols* reads, const uint32_t* cigar, int64_t n_cigar, const csv_sa_cols* sa,
+                             const csv_seq_cols* seq, const csv_name_cols* names, void* stream, int64_t counts[CSV_NTYPES],
+                             int64_t* n_read_rows);
+int csv_extract_append_named_device(csv_ctx* ctx, const csv_read_cols* reads, const uint32_t* cigar, int64_t n_cigar,
+                                    const csv_sa_cols* sa, const csv_seq_cols* seq, const csv_name_cols* names, void* stream,
+                                    int64_t counts[CSV_NTYPES], int64_t* n_read_rows);
+/* Sorts the names of a named accumulation byte-lexicographically (a proper prefix first, embedded NUL bytes included) on the
+ * device, gives every record the dense rank of its name among the distinct names (*n_distinct, may be NULL) and rewrites the
+ * read ids of all five signature types and of the reads table from provisional ids to ranks, with no host copy.  A second
+ * call only reports the count.  CSV_E_STATE when the device-resident rows are not a named accumulation (or an upload came
+ * since).  Its scratch is csv_sort_sigs' (never csv_cluster's inputs, results or captured graphs). */
+int csv_rank_names(csv_ctx* ctx, int64_t* n_distinct);
+/* Device pointer of the ranked accumulation's table record -> rank (int32, *n_records entries), e.g. to turn the provisional
+ * ids of a caller-built alignment table (csv_upload_alignments_device) into ranks with one gather.  Blocks until the table is
+ * complete; valid until the next extraction, csv_extract_reset or csv_destroy.  CSV_E_STATE before csv_rank_names. */
+int csv_name_ranks_device_ptr(csv_ctx* ctx, const int32_t** rank_of_record, int64_t* n_records);
+/* Names of ranks ranks[0..n) (any order, repeats allowed), gathered on the device, one D2H copy: rank ranks[i] is
+ * out[out_off[i] .. out_off[i + 1]) (out_off: n + 1 entries, 64-bit).  On CSV_E_CAPACITY out_off is filled and out_off[n]
+ * is the size `out` needs.  CSV_E_STATE before csv_rank_names, CSV_E_INVALID for a rank outside [0, n_distinct). */
+int csv_fetch_names(csv_ctx* ctx, const int32_t* ranks, int64_t n, uint8_t* out, int64_t cap, int64_t* out_off);
+/* Puts the INS rows that tie on (contig, int(pos), len, read) into the order of their sequence strings (cuteSV:774) on the
+ * device, from the sequence arena: each tie group's contents, ordered by (sequence bytes, row), go onto the group's rows in
+ * ascending order.  Moves everything csv_swap_ins_rows moves (and likewise invalidates the record column); the result equals
+ * the host's swaps (cutesv_b200/cli.py ins_tie_swaps) applied with csv_swap_ins_rows.  *n_rows_moved (may be NULL): rows whose
+ * content changed.
+ *   - CSV_E_STATE without a valid sequence arena: ties then keep extraction order (as with --ignore_sequence).
+ *   - The read ids must be final ranks.  For a named accumulation the call checks that csv_rank_names ran (CSV_E_STATE
+ *     otherwise); for any other accumulation that is the caller's contract, met by csv_remap_read_ids. */
+int csv_order_ins_ties(csv_ctx* ctx, int64_t* n_rows_moved);
+
 /* Records whose split-read analysis was skipped because they carry more than 64 qualifying segments (only reachable
  * with --max_split_parts -1; their CIGAR signatures are taken).  The reference has no such limit: a documented,
  * counted deviation instead of a failed run. */
