@@ -128,6 +128,7 @@ struct Lane {
     cudaEvent_t ev_join = nullptr;
     bool used = false;                  // forked from ev_fork in the call being enqueued
     bool prev_is_chain_kernel = false;  // the launch being enqueued directly follows a chain kernel on this stream
+    int mark = -1;                      // lane_marks: index of the open back-end interval in kivs
     DBuf keys_a, keys_b, vals_a, vals_b, hist, lb_status, big_list, giant_list, giant_arena;
     DBuf boff, rec_a, recc_a, rest_list;   // partitioned INS/DEL front end, k_cluster_small's rest list
     SmallWork small;
@@ -218,6 +219,9 @@ struct csv_ctx {
     int64_t launches = 0;
     // profiling: CUDA-event intervals on the launching streams; a stage may be entered once per SV type
     bool profiling = false;
+    // csv_set_profiling(c, 2): no per-launch events (programmatic launches, the side streams and the lanes run as they do
+    // unprofiled; no graph replay), only one interval per INS / DEL lane from the end of the density filter to the lane's end
+    bool lane_marks = false;
     struct Interval { int st; cudaEvent_t a, b; int64_t bytes; };
     std::vector<Interval> ivs;
     std::vector<cudaEvent_t> ev_pool;
@@ -616,7 +620,8 @@ extern "C" int csv_set_lanes(csv_ctx* c, int on) {
 extern "C" int csv_set_profiling(csv_ctx* c, int on) {
     if (!c) return set_err(CSV_E_INVALID, "null ctx");
     CU(cudaSetDevice(c->device));
-    c->profiling = on != 0;
+    c->profiling = on == 1;
+    c->lane_marks = on == 2;
     return CSV_OK;
 }
 
@@ -965,7 +970,7 @@ static int run_segment_and_cluster(csv_ctx* c, Lane& L, TypeJob& J, int t, uint3
     if ((J.cp.min_support + 31) / 32 + 1 <= HEAD_MAX_NEED_WORDS) {
         MemberRec MR;
         memset(&MR, 0, sizeof(MR));
-        J.small_list = nullptr; J.n_small = nullptr; J.rest_list = nullptr; J.n_rest = nullptr;
+        J.small_list = nullptr; J.n_small = nullptr; J.rest_list = nullptr; J.n_rest = nullptr; J.n_rest_lo = nullptr;
         if ((t == CSV_DEL || t == CSV_INS) && J.iv.rec) {
             MR.rec = const_cast<IndelRec*>(J.iv.rec); MR.recc = const_cast<int32_t*>(J.iv.recc);
             MR.a = J.iv.a; MR.b = J.iv.b; MR.rid = J.iv.rid; MR.c = J.iv.recc ? J.iv.c : nullptr; MR.sidx = J.iv.sidx;
@@ -973,15 +978,21 @@ static int run_segment_and_cluster(csv_ctx* c, Lane& L, TypeJob& J, int t, uint3
                 CU(L.rest_list.ensure((size_t)c->kept_cap[t] * 12 + 64));
                 MR.rest_list = L.rest_list.as<uint32_t>();
                 MR.small_list = (uint2*)(L.rest_list.as<uint32_t>() + c->kept_cap[t] + (c->kept_cap[t] & 1u));
-                if ((rc = take_ticket(c->lb, &MR.n_small)) || (rc = take_ticket(c->lb, &MR.n_rest))) return rc;
+                if ((rc = take_ticket(c->lb, &MR.n_small)) || (rc = take_ticket(c->lb, &MR.n_rest)) || (rc = take_ticket(c->lb, &MR.n_rest_lo)))
+                    return rc;
+                MR.rest_cap = c->kept_cap[t];
                 J.small_list = MR.small_list; J.n_small = MR.n_small; J.rest_list = MR.rest_list; J.n_rest = MR.n_rest;
+                J.n_rest_lo = MR.n_rest_lo; J.rest_cap = MR.rest_cap;
             }
         }
+        // every CTA that fits at once: the tiles' look-backs and member gathers are latency chains, so a CTA that waits
+        // should have others beside it (the survivors of the density filter are about a quarter of the bound n_host)
+        const int sel_grid = std::min(grid_for(c, J.n_host, SEL_TILE, 64), resident_grid(c, k_select_heads, SEL_THREADS, 0));
         if (L.prev_is_chain_kernel)   // directly behind k_part_filter on this stream
-            LAUNCH_PDL(c, s, k_select_heads, grid_for(c, J.n_host, SEL_TILE, 4), SEL_THREADS, 0, J, c->kept[t].as<uint32_t>(), c->kept_cap[t],
+            LAUNCH_PDL(c, s, k_select_heads, sel_grid, SEL_THREADS, 0, J, c->kept[t].as<uint32_t>(), c->kept_cap[t],
                        &ctr->n_kept[t], ts, &ctr->status, (uint32_t)ST_LIST_OVERFLOW, MR);
         else
-            LAUNCH(c, s, k_select_heads, grid_for(c, J.n_host, SEL_TILE, 4), SEL_THREADS, 0, J, c->kept[t].as<uint32_t>(), c->kept_cap[t],
+            LAUNCH(c, s, k_select_heads, sel_grid, SEL_THREADS, 0, J, c->kept[t].as<uint32_t>(), c->kept_cap[t],
                    &ctr->n_kept[t], ts, &ctr->status, (uint32_t)ST_LIST_OVERFLOW, MR);
     } else {
         J.iv.rec = nullptr; J.iv.recc = nullptr;   // generic path: members are gathered by the cluster kernels
@@ -1018,7 +1029,7 @@ static int run_segment_and_cluster(csv_ctx* c, Lane& L, TypeJob& J, int t, uint3
         if (t == CSV_INS) LAUNCH_PDL_NAMED(c, s, "k_cluster_small<INS>", (k_cluster_small<true>), c->n_sm * 6, 256, 0, JS, E, ctr, work_s, n_rest);
         else LAUNCH_PDL_NAMED(c, s, "k_cluster_small<DEL>", (k_cluster_small<false>), c->n_sm * 6, 256, 0, JS, E, ctr, work_s, n_rest);
         if (!J.small_list) { J.rest_list = JS.rest_list; J.n_rest = n_rest; }
-    } else { J.small_list = nullptr; J.n_small = nullptr; J.rest_list = nullptr; J.n_rest = nullptr; }
+    } else { J.small_list = nullptr; J.n_small = nullptr; J.rest_list = nullptr; J.n_rest = nullptr; J.n_rest_lo = nullptr; }
     switch (kind_of(t)) {   // one per-type routine per kernel instantiation (instruction-cache footprint)
         case 0:
             if (t == CSV_DEL) { if (keep_all) launch_cluster_kind<6, 0>(c, gs, J, E, ctr, work, smem_warp); else launch_cluster_kind<4, 0>(c, gs, J, E, ctr, work, smem_warp); }
@@ -1033,6 +1044,7 @@ static int run_segment_and_cluster(csv_ctx* c, Lane& L, TypeJob& J, int t, uint3
         CU(cudaStreamWaitEvent(s, c->ev_side_join[side_k], 0));
     }
     stage_end(c, s, CSV_ST_CLUSTER);
+    if (L.mark >= 0) { CU(cudaEventRecord(c->kivs[L.mark].b, s)); L.mark = -1; }
     return CSV_OK;
 }
 
@@ -1091,6 +1103,10 @@ static int run_indel(csv_ctx* c, Lane& L, int t, uint32_t kslot_base) {
         LAUNCH_PDL(c, st, k_part_filter, g, 256, smem, (const uint2*)pairs, (const uint32_t*)runs, n_chunks, P, W, rb, (uint32_t)J.cp.min_support,
                    (const uint32_t*)edge, L.keys_b.as<uint32_t>(), L.vals_b.as<uint32_t>(), (uint2*)L.rec_a.p, n_pass, ts);
         stage_end(c, st, CSV_ST_SORT);
+        if (c->lane_marks) {
+            kprof_begin(c, st, t == CSV_DEL ? "back end<DEL>" : "back end<INS>");
+            L.mark = (int)c->kivs.size() - 1;
+        }
         J.n_dev = n_pass;
         J.keys32 = L.keys_b.as<uint32_t>();
         sidx = L.vals_b.as<uint32_t>();
@@ -1480,7 +1496,7 @@ extern "C" int csv_cluster(csv_ctx* c, uint32_t type_mask) {
         pending |= c->up_pending[t];
     }
     bool done = false;
-    if (c->graphs_enabled && !c->profiling && !pending) {
+    if (c->graphs_enabled && !c->profiling && !c->lane_marks && !pending) {
         csv_ctx::GraphKey key;
         memset(&key, 0, sizeof(key));
         key.mask = type_mask;
@@ -1596,7 +1612,7 @@ extern "C" int csv_fetch(csv_ctx* c, csv_cand* cands, csv_geno* genos, int64_t c
     if (nn) CU(cudaMemcpyAsync(names, c->names.p, (size_t)nn * 4, cudaMemcpyDeviceToHost, c->stream));
     stage_end(c, c->stream, CSV_ST_D2H);
     CU(cudaStreamSynchronize(c->stream));
-    if (c->profiling) stage_collect(c);
+    if (c->profiling || c->lane_marks) stage_collect(c);
     return CSV_OK;
 }
 

@@ -41,6 +41,10 @@ struct TypeJob {
     int small_path;          // INS / DEL: clusters of <= 32 members go through the register kernel (k_cluster_small) first
     uint32_t* rest_list;     // ... which lists the others here (kept-cluster ordinals); null: the general kernel takes every cluster
     const uint32_t* n_rest;
+    // record mode: k_select_heads lists the clusters of more than REST_SPLIT members from the front of rest_list and the
+    // others from its end (rest_cap words), so that the general kernel hands out the costly clusters first
+    const uint32_t* n_rest_lo;
+    uint32_t rest_cap;
     uint2* small_list;       // (ordinal, members) of the clusters of <= 32 members, written by k_select_heads in record mode
     const uint32_t* n_small;
 };
@@ -94,8 +98,10 @@ struct MemberRec {
     const uint32_t* sidx;
     // classification of the kept clusters by size while their records are gathered (null: not wanted)
     uint2* small_list; uint32_t* n_small;    // (kept ordinal, members) for <= 32 members
-    uint32_t* rest_list; uint32_t* n_rest;   // kept ordinal for the others
+    uint32_t* rest_list; uint32_t* n_rest;   // kept ordinal for the others: > REST_SPLIT members from the front,
+    uint32_t* n_rest_lo; uint32_t rest_cap;  // ... the others from the end of the rest_cap words
 };
+static constexpr int REST_SPLIT = 64;
 __global__ void __launch_bounds__(SEL_THREADS) k_select_heads(TypeJob J, uint32_t* out, uint32_t out_cap, uint32_t* out_count,
                                                               TileSync ts, uint32_t* status_word, uint32_t overflow_bit, MemberRec MR) {
     pdl_launch_dependents(); pdl_wait();   // programmatic dependent launch: resident early, starts when the previous kernel has finished
@@ -103,8 +109,9 @@ __global__ void __launch_bounds__(SEL_THREADS) k_select_heads(TypeJob J, uint32_
     __shared__ uint32_t s_link[WORDS + HEAD_MAX_NEED_WORDS + 2];
     __shared__ uint32_t s_warp[9];
     __shared__ uint32_t s_tile, s_excl;
-    __shared__ uint32_t s_nheads;
+    __shared__ uint32_t s_nheads, s_hnext;
     __shared__ uint16_t s_heads[SEL_TILE];
+    __shared__ uint8_t s_msize[SEL_TILE];   // record mode: members of head h (<= 32), 33: up to REST_SPLIT, 34: more
     const int64_t n = job_n(J);
     const uint32_t gen = ts_gen(ts);
     const int need = J.cp.min_support;
@@ -155,6 +162,15 @@ __global__ void __launch_bounds__(SEL_THREADS) k_select_heads(TypeJob J, uint32_
         }
         uint32_t total;
         const uint32_t local = block_excl_scan_256(cnt, s_warp, &total);
+        if (MR.rec) {   // the tile's heads in order; the member gather needs their tile positions, not their ordinals
+            uint32_t o = local;
+#pragma unroll
+            for (int j = 0; j < SEL_ITEMS; j++)
+                if (flags >> j & 1u) s_heads[o++] = (uint16_t)(p0 + j);
+            if (threadIdx.x == 0) { s_nheads = total; s_hnext = 0; }
+            __syncthreads();
+        }
+        // warp 0 waits for the look-back while the other warps gather the members (it joins them afterwards)
         if (threadIdx.x < 32) {
             const uint32_t ex = lookback_exclusive_warp(ts.status, gen, (int)tile, total);
             if (threadIdx.x == 0) {
@@ -162,23 +178,14 @@ __global__ void __launch_bounds__(SEL_THREADS) k_select_heads(TypeJob J, uint32_
                 if (base + SEL_TILE >= n) *out_count = ex + total;
             }
         }
-        __syncthreads();
-        uint32_t o = s_excl + local;
-#pragma unroll
-        for (int j = 0; j < SEL_ITEMS; j++) {
-            if (flags >> j & 1u) {
-                if (o < out_cap) out[o] = (uint32_t)(base + p0 + j);
-                else atomicOr(status_word, overflow_bit);
-                if (MR.rec) s_heads[local + (o - (s_excl + local))] = (uint16_t)(p0 + j);
-                o++;
-            }
-        }
         if (MR.rec) {
-            if (threadIdx.x == 0) s_nheads = total;
-            __syncthreads();
             const uint32_t nh = s_nheads;
             uint32_t bad = 0;
-            for (uint32_t h = warp; h < nh; h += SEL_THREADS / 32) {
+            while (true) {
+                uint32_t h = 0;
+                if (lane == 0) h = atomicAdd(&s_hnext, 1u);
+                h = __shfl_sync(0xffffffffu, h, 0);
+                if (h >= nh) break;
                 const int64_t s0 = base + s_heads[h];
                 // members s0 .. s0+m-1: 32 links per step until the first missing one
                 int64_t done = 1;
@@ -199,10 +206,7 @@ __global__ void __launch_bounds__(SEL_THREADS) k_select_heads(TypeJob J, uint32_
                     if (bm) { done += take; break; }
                     done += 32;
                 }
-                if (MR.small_list && lane == 0) {   // `done` = members of the cluster; its kept ordinal = s_excl + h
-                    if (done <= 32) MR.small_list[atomicAdd(MR.n_small, 1u)] = make_uint2(s_excl + h, (uint32_t)done);
-                    else MR.rest_list[atomicAdd(MR.n_rest, 1u)] = s_excl + h;
-                }
+                if (lane == 0) s_msize[h] = (uint8_t)(done <= 32 ? done : done <= REST_SPLIT ? 33 : 34);
                 if (lane == 0) {   // the head itself
                     const uint32_t x = MR.sidx[s0];
                     IndelRec r;
@@ -214,6 +218,38 @@ __global__ void __launch_bounds__(SEL_THREADS) k_select_heads(TypeJob J, uint32_
                 }
             }
             if (bad) atomicOr(status_word, bad);
+        }
+        __syncthreads();
+        uint32_t o = s_excl + local;
+#pragma unroll
+        for (int j = 0; j < SEL_ITEMS; j++) {
+            if (flags >> j & 1u) {
+                if (o < out_cap) out[o] = (uint32_t)(base + p0 + j);
+                else atomicOr(status_word, overflow_bit);
+                o++;
+            }
+        }
+        if (MR.small_list) {   // the size lists of the cluster kernels, one atomic per warp and list; kept ordinal = s_excl + h
+            const uint32_t nh = s_nheads, ex = s_excl;
+            for (uint32_t h0 = warp * 32; h0 < nh; h0 += SEL_THREADS) {
+                const uint32_t h = h0 + lane;
+                const uint32_t sz = h < nh ? s_msize[h] : 255u;
+                const uint32_t lt = (1u << lane) - 1u;
+                const uint32_t m_small = __ballot_sync(0xffffffffu, sz <= 32u);
+                const uint32_t m_lo = __ballot_sync(0xffffffffu, sz == 33u), m_hi = __ballot_sync(0xffffffffu, sz == 34u);
+                uint32_t b_small = 0, b_lo = 0, b_hi = 0;
+                if (lane == 0) {
+                    if (m_small) b_small = atomicAdd(MR.n_small, (uint32_t)__popc(m_small));
+                    if (m_lo) b_lo = atomicAdd(MR.n_rest_lo, (uint32_t)__popc(m_lo));
+                    if (m_hi) b_hi = atomicAdd(MR.n_rest, (uint32_t)__popc(m_hi));
+                }
+                b_small = __shfl_sync(0xffffffffu, b_small, 0);
+                b_lo = __shfl_sync(0xffffffffu, b_lo, 0);
+                b_hi = __shfl_sync(0xffffffffu, b_hi, 0);
+                if (sz <= 32u) MR.small_list[b_small + __popc(m_small & lt)] = make_uint2(ex + h, sz);
+                else if (sz == 33u) MR.rest_list[MR.rest_cap - 1u - (b_lo + __popc(m_lo & lt))] = ex + h;
+                else if (sz == 34u) MR.rest_list[b_hi + __popc(m_hi & lt)] = ex + h;
+            }
         }
         __syncthreads();
     }
@@ -980,7 +1016,8 @@ __global__ void __launch_bounds__(CL_THREADS) k_cluster_warp(TypeJob J, Emit E, 
     char* arena = smem + (size_t)warp * (WARP_M * ARENA_PER_MAX);
     int64_t* red = (int64_t*)(smem + (size_t)WARPS * (WARP_M * ARENA_PER_MAX)) + warp * 40;
     const int64_t n = job_n(J);
-    const uint32_t n_kept = J.rest_list ? *J.n_rest : ctr->n_kept[J.svtype];
+    const uint32_t n_hi = J.rest_list ? *J.n_rest : ctr->n_kept[J.svtype];
+    const uint32_t n_kept = n_hi + (J.n_rest_lo ? *J.n_rest_lo : 0u);
     CudaTeam<32> tm;
     // dynamic hand-out (one atomic per cluster): cluster costs vary, a static stride leaves a long tail
     // (the ticket of the NEXT cluster is requested before the current one is processed, so the atomic's round
@@ -991,7 +1028,8 @@ __global__ void __launch_bounds__(CL_THREADS) k_cluster_warp(TypeJob J, Emit E, 
         const uint32_t q = __shfl_sync(0xffffffffu, k_next, 0);
         if (q >= n_kept) break;
         if (lane == 0) k_next = atomicAdd(work, 1u);
-        const uint32_t k = J.rest_list ? J.rest_list[q] : q;   // after k_cluster_small: only the clusters it left
+        // after k_cluster_small: only the clusters it left, the larger ones first
+        const uint32_t k = !J.rest_list ? q : q < n_hi ? J.rest_list[q] : J.rest_list[J.rest_cap - 1u - (q - n_hi)];
         const int64_t s = J.kept_start[k];
         const int m = cluster_size_warp(J, s, n, WARP_M);
         if (m > WARP_M) {

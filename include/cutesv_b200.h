@@ -489,7 +489,9 @@ int csv_fetch_pieces(csv_ctx* ctx, int64_t cap, int32_t* pieces4, int64_t* n_pie
 int csv_fetch_read_rows(csv_ctx* ctx, int64_t cap, int32_t* chrom, int32_t* start, int32_t* end,
                         int32_t* read_id, uint8_t* is_primary);
 
-/* Profiling: per-stage device milliseconds of the last csv_cluster / csv_extract call. */
+/* Profiling: per-stage device milliseconds of the last csv_cluster / csv_extract call.  on = 2: no per-launch events and
+ * no graph replay, only one interval per INS / DEL lane that takes the density filter, from the filter's end to the
+ * lane's end, reported by csv_kernel_times as "back end<DEL>" / "back end<INS>". */
 int csv_set_profiling(csv_ctx* ctx, int on);
 int csv_stage_ms(csv_ctx* ctx, float ms[CSV_ST_COUNT]);
 /* Per-kernel totals of the last profiled call(s): with profiling on, every kernel launch sits between its own
