@@ -336,6 +336,38 @@ def device_packet(packet, device):
     return out
 
 
+def scan_packet(packet, device):
+    """device_packet of a scanned packet (csv_scan_append_named_device): every decoded record of a BAM packet, in GPU memory and
+    with names / name_off.  Raises what device_packet raises, and ValueError for a host packet or a packet without names."""
+    d = device_packet(packet, device)
+    if d is None:
+        raise ValueError("a scanned packet lives in GPU memory (torch CUDA tensors); host packets go through extract()")
+    if d.names is None:
+        raise ValueError("a scanned packet carries names / name_off: the library numbers its records and ranks their names")
+    return d
+
+
+def scan_regions(tasks, bed, chrom_id):
+    """Arrays of csv_set_scan_regions from cli.task_windows' tasks ([contig, start, end], start may be a float), cli.load_bed's
+    region lists (one list of (lo, hi) per task, or None: no table) and the contig ids: (n_contigs, win_off int64, win_start float64,
+    reg_off int64, reg int64 [n_regions, 2]).  n_contigs is 0 without a BED file.  A contig's windows keep their task order."""
+    if bed is None:
+        return 0, None, None, None, None
+    if len(bed) != len(tasks):
+        raise ValueError("bed has %d region lists for %d tasks" % (len(bed), len(tasks)))
+    n_contigs = max(chrom_id.values()) + 1 if chrom_id else 0
+    cid = np.array([chrom_id[t[0]] for t in tasks], dtype=np.int64)
+    order = np.argsort(cid, kind="stable")
+    win_off = np.zeros(n_contigs + 1, dtype=np.int64)
+    np.cumsum(np.bincount(cid, minlength=n_contigs), out=win_off[1:])
+    win_start = np.array([tasks[i][1] for i in order.tolist()], dtype=np.float64)
+    regs = [bed[i] for i in order.tolist()]
+    reg_off = np.zeros(len(tasks) + 1, dtype=np.int64)
+    np.cumsum([len(r) for r in regs], out=reg_off[1:])
+    reg = np.array([x for r in regs for x in r], dtype=np.int64).reshape(-1, 2)
+    return n_contigs, win_off, win_start, reg_off, reg
+
+
 def default_params(**kw):
     """Reference defaults (cuteSV_Description.py:78-262; wiring cuteSV:1116-1189)."""
     p = csv_params()

@@ -66,6 +66,10 @@ _SIGNATURES = {
     "csv_name_ranks_device_ptr": (C.c_int, [_VP, C.POINTER(_VP), _I64P]),
     "csv_fetch_names": (C.c_int, [_VP, _I32P, C.c_int64, C.POINTER(C.c_uint8), C.c_int64, _I64P]),
     "csv_order_ins_ties": (C.c_int, [_VP, _I64P]),
+    "csv_fetch_alignments": (C.c_int, [_VP, C.c_int64, _I32P, _I32P, _I32P, _I32P, C.POINTER(C.c_uint8), _I64P]),
+    "csv_set_scan_regions": (C.c_int, [_VP, C.c_int32, _I64P, C.POINTER(C.c_double), _I64P, _I64P]),
+    "csv_scan_append_named_device": (C.c_int, [_VP, C.POINTER(_abi.csv_read_cols), C.POINTER(C.c_uint32), C.c_int64, C.POINTER(_abi.csv_sa_cols),
+                                               C.POINTER(_abi.csv_seq_cols), C.POINTER(_abi.csv_name_cols), C.c_int, _VP, _I64P, _I64P, _I64P]),
     "csv_ins_seq_device_ptrs": (C.c_int, [_VP, C.POINTER(_VP), C.POINTER(_VP), C.POINTER(_VP), _I64P]),
     "csv_fetch_ins_seqs": (C.c_int, [_VP, _I64P, C.c_int64, C.POINTER(C.c_uint8), C.c_int64, _I64P]),
     "csv_extract_reset": (C.c_int, [_VP]),

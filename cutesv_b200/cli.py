@@ -439,11 +439,7 @@ class _NativeSource(object):
     def scan(self, args, eng, acc, tasks, bed, chrom_id, want_seq):
         bamio, rd = self.bamio, self.rd
         rd.set_chrom_ids(chrom_id)
-        # window starts per contig id -> owning task of a record (only the bed filter needs it)
-        starts, first_task = {}, {}
-        for i, t in enumerate(tasks):
-            starts.setdefault(chrom_id[t[0]], []).append(t[1])
-            first_task.setdefault(chrom_id[t[0]], i)
+        starts, first_task = window_starts(tasks, chrom_id)
         n_seen = 0
         while True:
             pk = rd.next_packet(PACKET_READS, copy=False)   # views: everything kept beyond this iteration is copied below
@@ -456,17 +452,7 @@ class _NativeSource(object):
                                         ((pk["flag"][v] == 0) | (pk["flag"][v] == 16)).astype(np.uint8))
             keep = has_cigar & (pk["flag"] != 256) & (pk["flag"] != 272) & (pk["chrom"] >= 0)
             if bed is not None:
-                owner = np.zeros(len(keep), dtype=np.int64)
-                for c in np.unique(pk["chrom"]):
-                    m = pk["chrom"] == c
-                    if int(c) in starts:
-                        owner[m] = first_task[int(c)] + np.searchsorted(np.asarray(starts[int(c)], dtype=np.float64), pk["ref_start"][m], side="right") - 1
-                for ti in np.unique(owner[keep]):
-                    m = keep & (owner == ti)
-                    hit = np.zeros(len(keep), dtype=bool)
-                    for r in bed[int(ti)]:
-                        hit |= ~((pk["ref_end"] <= r[0]) | (pk["ref_start"] >= r[1]))
-                    keep[m & ~hit] = False
+                bed_filter(pk, keep, bed, starts, first_task)
             sub = bamio.subset_packet(pk, np.flatnonzero(keep))
             if len(sub["chrom"]):
                 last = [-1, ""]   # the INS signatures of one record follow each other: decode its query once
@@ -480,6 +466,31 @@ class _NativeSource(object):
             n_seen += len(keep)
             logging.info("Decoded %d records." % n_seen)
         return rd.names(), rd.name_ranks()
+
+
+def window_starts(tasks, chrom_id):
+    """Window starts per contig id and the index of each contig's first task: what bed_filter needs to find a record's window."""
+    starts, first_task = {}, {}
+    for i, t in enumerate(tasks):
+        starts.setdefault(chrom_id[t[0]], []).append(t[1])
+        first_task.setdefault(chrom_id[t[0]], i)
+    return starts, first_task
+
+
+def bed_filter(pk, keep, bed, starts, first_task):
+    """-include_bed on one decoded packet: clears keep[i] of every kept record that overlaps no padded region of the window owning
+    it, the last window of its contig starting at or before its ref_start (cuteSV:725)."""
+    owner = np.zeros(len(keep), dtype=np.int64)
+    for c in np.unique(pk["chrom"]):
+        m = pk["chrom"] == c
+        if int(c) in starts:
+            owner[m] = first_task[int(c)] + np.searchsorted(np.asarray(starts[int(c)], dtype=np.float64), pk["ref_start"][m], side="right") - 1
+    for ti in np.unique(owner[keep]):
+        m = keep & (owner == ti)
+        hit = np.zeros(len(keep), dtype=bool)
+        for r in bed[int(ti)]:
+            hit |= ~((pk["ref_end"] <= r[0]) | (pk["ref_start"] >= r[1]))
+        keep[m & ~hit] = False
 
 
 class _NameIds(object):

@@ -23,6 +23,7 @@
 #include "kernels.cuh"
 #include "radix.cuh"
 #include "extract.cuh"
+#include "scan_core.h"
 
 using namespace csv;
 
@@ -116,6 +117,15 @@ struct ExtractState {
     bool named = false;              // every packet of the accumulation carried names
     bool ranked = false;             // csv_rank_names has turned the provisional ids into ranks
     int64_t name_nbytes = 0, n_names = 0;
+    // scanned accumulation (csv_scan_append_named_device, scan_api.inl): every decoded record of each packet.  scan_flag is the
+    // packet's flag column with 256 on every record the reference would not extract; p_* the pending alignment table (BAM
+    // order, provisional ids) that csv_rank_names installs; rg_* the region table of csv_set_scan_regions.
+    DBuf scan_flag, scan_excl, p_chrom, p_start, p_end, p_id, p_prim;
+    DBuf rg_win_off, rg_win_start, rg_reg_off, rg_reg;
+    bool scanned = false;            // every packet of the accumulation was scanned
+    bool scan_aln = false;           // ... and asked for alignment rows
+    int64_t n_pending = 0;
+    int32_t rg_n_contigs = 0;        // 0: no region table
     double per_record[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // largest yield of a packet so far: signatures per type [0..4], pieces [5] per alignment record
 };
 
@@ -718,6 +728,7 @@ static int upload_sigs_impl(csv_ctx* c, int t, const csv_sig_cols* h, const int6
     c->ex.rec_valid = false;
     c->ex.seq_valid = false;
     c->ex.named = false; c->ex.ranked = false;   // the rows no longer come from the named accumulation
+    c->ex.scanned = false; c->ex.n_pending = 0;
     c->up_checked[t] = false;
     if (h->n == 0) return CSV_OK;
     if ((!contig_off && !h->chrom) || !h->a || !h->b || !h->read_id) return set_err(CSV_E_INVALID, "null column");
@@ -763,6 +774,7 @@ static int upload_reads_impl(csv_ctx* c, const csv_reads_cols* h, const int64_t*
     c->ex.rec_valid = false;
     c->ex.seq_valid = false;
     c->ex.named = false; c->ex.ranked = false;   // the rows no longer come from the named accumulation
+    c->ex.scanned = false; c->ex.n_pending = 0;
     c->up_checked[CSV_NTYPES] = false;
     if (h->n == 0) return CSV_OK;
     if ((!contig_off && !h->chrom) || !h->start || !h->end || !h->read_id || !h->is_primary) return set_err(CSV_E_INVALID, "null column");
@@ -800,6 +812,26 @@ extern "C" int csv_upload_reads_grouped_device(csv_ctx* c, const csv_reads_cols*
     return upload_reads_impl(c, d, contig_off, UpSrc{true, (cudaStream_t)stream});
 }
 
+// Contig index + sortedness check of the n rows in c->a_* (BAM order is a precondition of the early-exit scan); one
+// synchronisation.  A failure leaves no table.
+static int aln_index(csv_ctx* c, int64_t n) {
+    CU(c->aln_flag.ensure(64));
+    uint32_t* flag = c->aln_flag.as<uint32_t>();
+    CU(cudaMemsetAsync(flag, 0, 4, c->stream));
+    CU(cudaMemsetAsync(c->a_span.p, 0, ((size_t)c->n_contigs + 2) * 4, c->stream));
+    LAUNCH(c, c->stream, k_aln_index, grid_for(c, n, 256), 256, 0, c->a_chrom.as<int32_t>(), c->a_start.as<int32_t>(), c->a_end.as<int32_t>(), n,
+           c->n_contigs, c->a_span.as<int32_t>(), flag);
+    LAUNCH(c, c->stream, k_aln_off, grid_for(c, (int64_t)c->n_contigs + 1, 256), 256, 0, c->a_chrom.as<int32_t>(), n, c->n_contigs, c->a_off.as<uint32_t>());
+    uint32_t hflag = 0;
+    CU(cudaMemcpyAsync(&hflag, flag, 4, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    if (hflag) {
+        c->n_aln = 0;
+        return set_err(CSV_E_INPUT, "alignment table: %s", (hflag & ST_UNSORTED) ? "not coordinate-sorted (BAM order required)" : "contig id out of range");
+    }
+    return CSV_OK;
+}
+
 // The alignment table is copied on the ctx stream and its order is checked before the call returns (one synchronisation, for host
 // and device columns alike), so a device source's buffers are free again on return.
 static int upload_alignments_impl(csv_ctx* c, const csv_reads_cols* h, const UpSrc& src) {
@@ -809,6 +841,7 @@ static int upload_alignments_impl(csv_ctx* c, const csv_reads_cols* h, const UpS
     CU(cudaSetDevice(c->device));
     c->n_aln = h->n;
     c->counts_valid = false;
+    c->ex.scanned = false; c->ex.n_pending = 0;   // the table no longer comes from a scanned accumulation
     if (h->n == 0) return CSV_OK;
     if (!h->chrom || !h->start || !h->end || !h->read_id || !h->is_primary) return set_err(CSV_E_INVALID, "null column");
     if (src.device) {
@@ -831,22 +864,7 @@ static int upload_alignments_impl(csv_ctx* c, const csv_reads_cols* h, const UpS
     CU(cudaMemcpyAsync(c->a_end.p, h->end, bytes, kind, c->stream));
     CU(cudaMemcpyAsync(c->a_id.p, h->read_id, bytes, kind, c->stream));
     CU(cudaMemcpyAsync(c->a_prim.p, h->is_primary, (size_t)h->n, kind, c->stream));
-    // contig index + sortedness check (BAM order is a precondition of the early-exit scan)
-    CU(c->aln_flag.ensure(64));
-    uint32_t* flag = c->aln_flag.as<uint32_t>();
-    CU(cudaMemsetAsync(flag, 0, 4, c->stream));
-    CU(cudaMemsetAsync(c->a_span.p, 0, ((size_t)c->n_contigs + 2) * 4, c->stream));
-    LAUNCH(c, c->stream, k_aln_index, grid_for(c, h->n, 256), 256, 0, c->a_chrom.as<int32_t>(), c->a_start.as<int32_t>(), c->a_end.as<int32_t>(), h->n,
-           c->n_contigs, c->a_span.as<int32_t>(), flag);
-    LAUNCH(c, c->stream, k_aln_off, grid_for(c, (int64_t)c->n_contigs + 1, 256), 256, 0, c->a_chrom.as<int32_t>(), h->n, c->n_contigs, c->a_off.as<uint32_t>());
-    uint32_t hflag = 0;
-    CU(cudaMemcpyAsync(&hflag, flag, 4, cudaMemcpyDeviceToHost, c->stream));
-    CU(cudaStreamSynchronize(c->stream));
-    if (hflag) {
-        c->n_aln = 0;
-        return set_err(CSV_E_INPUT, "alignment table: %s", (hflag & ST_UNSORTED) ? "not coordinate-sorted (BAM order required)" : "contig id out of range");
-    }
-    return CSV_OK;
+    return aln_index(c, h->n);
 }
 extern "C" int csv_upload_alignments(csv_ctx* c, const csv_reads_cols* h) { return upload_alignments_impl(c, h, HOST_SRC); }
 extern "C" int csv_upload_alignments_device(csv_ctx* c, const csv_reads_cols* d, void* stream) {
@@ -1716,8 +1734,13 @@ extern "C" int csv_sort_probe(csv_ctx* c, float* ms_total, int64_t* bytes_total,
     return CSV_OK;
 }
 
+// scan_api.inl: the scan's per-packet step inside extract_impl and the alignment table csv_rank_names installs
+static int scan_packet(csv_ctx* c, const csv_read_cols* reads, bool want_aln, int64_t* n_aln_new);
+static int scan_install_alignments(csv_ctx* c, cudaStream_t st, LbPool& lb);
+
 #include "extract_api.inl"
 #include "gather_api.inl"
 #include "genotype_api.inl"
 #include "sigsort_api.inl"
 #include "names_api.inl"
+#include "scan_api.inl"

@@ -477,6 +477,11 @@ def _extract_method(self, packed, append=False, stream=None):
         cig = np.ascontiguousarray(packed["cigar"], dtype=np.uint32)
         fn = self.L.csv_extract_append if append else self.L.csv_extract
         _lib.check(fn(self.h, C.byref(rc_), cig.ctypes.data_as(C.POINTER(C.c_uint32)), C.c_int64(len(cig)), C.byref(sa_), counts, C.byref(n_rows)))
+    return _extracted(self, counts, n_rows, append, first, first_rows, first_pieces)
+
+
+def _extracted(self, counts, n_rows, append, first, first_rows, first_pieces):
+    """Bookkeeping after an extraction call and extract()'s result."""
     self._ex_counts = [int(x) for x in counts]
     self._ex_rows = int(n_rows.value)
     self._dev_rows = self._ex_counts + [self._ex_rows]
@@ -487,6 +492,58 @@ def _extract_method(self, packed, append=False, stream=None):
     return dict(counts={name: int(counts[t]) for t, name in enumerate(_abi.TYPE_NAMES)}, n_rows=int(n_rows.value),
                 first={name: first[t] for t, name in enumerate(_abi.TYPE_NAMES)}, first_rows=first_rows, first_pieces=first_pieces,
                 n_pieces=self._ex_pieces)
+
+
+def _set_scan_regions_method(self, tasks, bed, chrom_id):
+    """Region table of the following scan() calls (csv_set_scan_regions) from cli.task_windows' tasks, cli.load_bed's region lists
+    and the contig ids; bed None clears it.  With a table, scan() extracts only the records the CLI keeps with -include_bed."""
+    n, win_off, win_start, reg_off, reg = _abi.scan_regions(tasks, bed, chrom_id)
+    if n == 0:
+        _lib.check(self.L.csv_set_scan_regions(self.h, C.c_int32(0), None, None, None, None))
+        return
+    _lib.check(self.L.csv_set_scan_regions(self.h, C.c_int32(n), win_off.ctypes.data_as(C.POINTER(C.c_int64)),
+                                           win_start.ctypes.data_as(C.POINTER(C.c_double)), reg_off.ctypes.data_as(C.POINTER(C.c_int64)),
+                                           reg.ctypes.data_as(C.POINTER(C.c_int64))))
+
+
+def _fetch_alignments_method(self):
+    """D2H of csv_cluster's alignment table (upload_alignments, or installed by rank_names after scan(..., alignments=True)):
+    dict(chrom, start, end, read_id, is_primary) in the table's order, or None when there is none."""
+    n = C.c_int64(0)
+    rc = self.L.csv_fetch_alignments(self.h, C.c_int64(0), None, None, None, None, None, C.byref(n))
+    if rc != _abi.CSV_E_CAPACITY:   # the size probe
+        _lib.check(rc)
+    if n.value == 0:
+        return None
+    k = n.value
+    cols = {c: np.zeros(k, dtype=np.int32) for c in ("chrom", "start", "end", "read_id")}
+    cols["is_primary"] = np.zeros(k, dtype=np.uint8)
+    _lib.check(self.L.csv_fetch_alignments(self.h, C.c_int64(k), *[_abi.ptr(cols[c]) for c in ("chrom", "start", "end", "read_id")],
+                                           cols["is_primary"].ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(n)))
+    return cols
+
+
+def _scan_method(self, packet, alignments=False, stream=None):
+    """Appends every decoded record of a BAM packet (csv_scan_append_named_device): a torch CUDA packet with names / name_off and
+    no read_id (_abi.scan_packet).  The library drops what the reference's single_pipe drops (no CIGAR, contig < 0, flag 256 or
+    272, outside the set_scan_regions table) and extracts the rest in place; alignments=True also keeps every record with a CIGAR
+    and a contig as a row of the TRA genotyper's alignment table, which rank_names() installs.  Record numbers (provisional ids,
+    name_rank_tensor, fetch_records, INS pieces) count all scanned records.  Returns extract()'s dict plus n_aln_rows."""
+    d = _abi.scan_packet(packet, self.device)
+    rc_, cig_p, n_cig, sa_, seq = d
+    appending = getattr(self, "_ex_appending", False)
+    first = list(getattr(self, "_ex_counts", [0] * _abi.CSV_NTYPES)) if appending else [0] * _abi.CSV_NTYPES
+    first_rows = getattr(self, "_ex_rows", 0) if appending else 0
+    first_pieces = getattr(self, "_ex_pieces", 0) if appending else 0
+    counts = (C.c_int64 * _abi.CSV_NTYPES)()
+    n_rows, n_aln = C.c_int64(0), C.c_int64(0)
+    st = self._producer_stream(stream, [packet])
+    _lib.check(self.L.csv_scan_append_named_device(self.h, C.byref(rc_), cig_p, C.c_int64(n_cig), C.byref(sa_),
+                                                   C.byref(seq) if seq is not None else None, C.byref(d.names), int(bool(alignments)),
+                                                   C.c_void_p(st or None), counts, C.byref(n_rows), C.byref(n_aln)))
+    out = _extracted(self, counts, n_rows, True, first, first_rows, first_pieces)
+    out["n_aln_rows"] = int(n_aln.value)
+    return out
 
 
 def _fetch_ins_seqs_method(self, rows):
@@ -526,7 +583,9 @@ def _ins_seq_tensors_method(self):
 
 def _rank_names_method(self):
     """Ranks the read names of a named accumulation on the device (csv_rank_names): every signature's and reads row's read id
-    becomes the dense rank of its name in byte (for UTF-8: Python str) order.  Returns the number of distinct names."""
+    becomes the dense rank of its name in byte (for UTF-8: Python str) order.  After scan(..., alignments=True) it also installs
+    the scanned alignment rows, ids as ranks and sorted by contig, as the TRA genotyper's table.  Returns the number of distinct
+    names."""
     nd = C.c_int64(0)
     _lib.check(self.L.csv_rank_names(self.h, C.byref(nd)))
     return int(nd.value)
@@ -676,3 +735,6 @@ Engine.rank_names = _rank_names_method
 Engine.fetch_names = _fetch_names_method
 Engine.name_rank_tensor = _name_rank_tensor_method
 Engine.order_ins_ties = _order_ins_ties_method
+Engine.set_scan_regions = _set_scan_regions_method
+Engine.fetch_alignments = _fetch_alignments_method
+Engine.scan = _scan_method

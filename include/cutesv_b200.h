@@ -447,6 +447,47 @@ int csv_fetch_names(csv_ctx* ctx, const int32_t* ranks, int64_t n, uint8_t* out,
  *     otherwise); for any other accumulation that is the caller's contract, met by csv_remap_read_ids. */
 int csv_order_ins_ties(csv_ctx* ctx, int64_t* n_rows_moved);
 
+/* ---- scanned packets: every decoded record, filtered on the device ----
+ * A caller that decodes a BAM into GPU memory hands over every record of a packet in BAM order, with names; the library
+ * applies the reference's record filter (single_pipe, cuteSV:697-733), the -include_bed test and builds the TRA genotyper's
+ * all-alignments table on the device.
+ *
+ * Region table (the task windows and -include_bed regions of cutesv_b200/cli.py task_windows + load_bed), host arrays:
+ *   - win_off: n_contigs + 1 offsets; the windows of contig id k are [win_off[k], win_off[k + 1]), their starts win_start[]
+ *     (float64: the reference's bounds may be fractional, cuteSV:1026-1034) ascending;
+ *   - reg_off: n_windows + 1 offsets (n_windows = win_off[n_contigs]); the padded regions of window w are the int64 (lo, hi)
+ *     pairs reg[2k], reg[2k + 1] for k in [reg_off[w], reg_off[w + 1]) (lo may be negative).
+ * n_contigs == 0 clears the table: no region filtering.  A record is kept iff, in its contig's last window starting at or
+ * before its ref_start (compared as float64), some region has not (ref_end <= lo or ref_start >= hi).  With a table, a record
+ * on a contig without a window is not extracted (the reference never fetches it).  CSV_E_INVALID for offsets that decrease or
+ * starts that are not ascending; CSV_E_STATE, changing nothing, while a scanned accumulation is open (appended to and not
+ * ranked). */
+int csv_set_scan_regions(csv_ctx* ctx, int32_t n_contigs, const int64_t* win_off, const double* win_start, const int64_t* reg_off,
+                         const int64_t* reg);
+/* Appends one scanned packet: the columns of csv_extract_append_named_device (device memory, checked the same way, CSV_E_INPUT
+ * changing nothing), but the packet holds every decoded record, in BAM order.
+ *   - Alignment row: every record with cigar_off[i + 1] > cigar_off[i] and chrom >= 0, as (chrom, ref_start, ref_end,
+ *     provisional id, is_primary = flag is 0 or 16), kept in a ctx-owned pending table, only when want_alignments != 0.
+ *   - Extracted: an alignment row whose flag is neither 256 nor 272 (exact values, cuteSV:711) and that passes the region
+ *     table.  The other records yield no signature and no reads row.
+ *   - Every record's name joins the name arena, so csv_rank_names ranks the names of all decoded records.
+ *   - Numbering: every per-record number refers to the record's index among all scanned records of the accumulation (the
+ *     packets the caller holds): provisional ids, csv_name_ranks_device_ptr, csv_fetch_records and the record of an INS piece.
+ *   - counts / n_read_rows as for csv_extract_append; *n_aln_rows (may be NULL): pending alignment rows so far.
+ *   - CSV_E_STATE, changing nothing: a scanned packet appended to an accumulation of other packets or the reverse, packets
+ *     that disagree on want_alignments, any append after csv_rank_names.  An upload of signatures, reads or alignments ends
+ *     the scanned state.
+ * csv_rank_names on a scanned accumulation that asked for alignments also turns the pending rows' ids into ranks, stable-sorts
+ * the rows by contig id on the device and installs them as csv_cluster's alignment table, checked as csv_upload_alignments
+ * checks a table: rows out of BAM order are CSV_E_INPUT, and the accumulation then stays unranked. */
+int csv_scan_append_named_device(csv_ctx* ctx, const csv_read_cols* reads, const uint32_t* cigar, int64_t n_cigar, const csv_sa_cols* sa,
+                                 const csv_seq_cols* seq, const csv_name_cols* names, int want_alignments, void* stream,
+                                 int64_t counts[CSV_NTYPES], int64_t* n_read_rows, int64_t* n_aln_rows);
+/* D2H of csv_cluster's alignment table, uploaded or installed by csv_rank_names (*n_rows: its row count, also on
+ * CSV_E_CAPACITY); any column pointer may be NULL. */
+int csv_fetch_alignments(csv_ctx* ctx, int64_t cap, int32_t* chrom, int32_t* start, int32_t* end, int32_t* read_id, uint8_t* is_primary,
+                         int64_t* n_rows);
+
 /* Records whose split-read analysis was skipped because they carry more than 64 qualifying segments (only reachable
  * with --max_split_parts -1; their CIGAR signatures are taken).  The reference has no such limit: a documented,
  * counted deviation instead of a failed run. */
