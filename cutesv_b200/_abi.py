@@ -207,21 +207,7 @@ def device_cols(cols, fields, device, grouped=False, n_contigs=None):
                          % (sorted(f for f, d in on_dev.items() if not d), sorted(f for f, d in on_dev.items() if d)))
     ptrs, lens = {}, {}
     for f, v in present.items():
-        cai = v.__cuda_array_interface__
-        want = _TYPESTR.get(f, "<i4")
-        if cai["typestr"] != want:
-            raise TypeError("column %s: dtype %s, expected %s" % (f, cai["typestr"], want))
-        shape = tuple(cai["shape"])
-        if len(shape) != 1:
-            raise TypeError("column %s: shape %s, expected one dimension" % (f, shape))
-        strides = cai.get("strides")
-        if strides is not None and shape[0] > 1 and tuple(strides) != (_ITEMSIZE[want],):
-            raise TypeError("column %s is not contiguous (strides %s)" % (f, tuple(strides)))
-        idx = _device_index(v)
-        if idx is not None and idx != device:
-            raise ValueError("column %s is on device %d, the engine on device %d" % (f, idx, device))
-        ptrs[f] = int(cai["data"][0]) if shape[0] else None
-        lens[f] = shape[0]
+        ptrs[f], lens[f] = _cai_check(f, v, (_TYPESTR.get(f, "<i4"),), device)
     row_cols = {f: n for f, n in lens.items() if f != "contig_off"}
     if len(set(row_cols.values())) > 1:
         raise ValueError("column lengths disagree: %s" % row_cols)

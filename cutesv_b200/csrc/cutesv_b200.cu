@@ -96,12 +96,31 @@ struct SmallWork {  // DUP / INV / TRA
     DBuf k_rid, k_b, k_prim, perm_a, perm_b, sel, u_chrom, u_a, u_b, u_rid, u_c;
 };
 
+// What the packets of an accumulation are; every packet of one accumulation is of one kind.  Named: the records carry read
+// names instead of read ids (csv_extract*_named_device); scanned: every decoded record of a BAM packet
+// (csv_scan_append_named_device, always named), with or without the alignment rows.
+enum class PacketKind { PLAIN, NAMED, SCANNED, SCANNED_ALN };
+static inline bool kind_named(PacketKind k) { return k != PacketKind::PLAIN; }
+static inline bool kind_scanned(PacketKind k) { return k == PacketKind::SCANNED || k == PacketKind::SCANNED_ALN; }
+
+// Pinned staging of the extraction stage's small copies, one field per use
+struct ExStaging {
+    uint32_t out[16];        // k_extract's counters, read back
+    uint32_t base[16];       // the counters at the start of a packet, H2D (a rerun must not race the previous copy)
+    uint32_t seq[8];         // the sequence builder's words [0, 8), read back
+    uint32_t bad;            // k_check_packet's error word
+    int64_t name_span[2];    // a named packet's name_off[0] and name_off[n]
+};
+
+// Words of ExtractState::seq_words (the sequence builder, seq_scan and k_check_packet; zeroed before each use)
+enum : int { SW_TICKET = 0, SW_TOTAL = 1, SW_STATUS = 2, SW_TOTAL64 = 4, SW_EPOCH = 8, SW_WORDS = 16 };
+
 struct ExtractState {
     DBuf r[7], cigar_off, sa_off, cigar, s[7], piece_off, piece_cnt, pieces, counters;
     DBuf rec[CSV_NTYPES + 1];        // record index of every extracted signature per type / reads row (last)
     bool rec_on = false;             // csv_extract_records: store the record column (off: no allocation, no stores)
     bool rec_valid = false;          // the device-resident rows are csv_extract* output with the column stored for all of them
-    uint32_t* h_counters = nullptr;  // pinned
+    ExStaging* h = nullptr;          // pinned
     uint32_t n_pieces = 0;
     uint32_t n_records = 0;          // alignment records of all packets of the accumulation (record index base of INS pieces)
     uint32_t n_skipped = 0;
@@ -114,7 +133,7 @@ struct ExtractState {
     // [name_off[i], name_off[i + 1]); the records' provisional read ids are their indices.  csv_rank_names adds the tables
     // record -> dense rank and rank -> (start, length).
     DBuf name_bytes, name_off, pid, name_rank, name_tab_start, name_tab_len, name_words;
-    bool named = false;              // every packet of the accumulation carried names
+    PacketKind kind = PacketKind::PLAIN;
     bool ranked = false;             // csv_rank_names has turned the provisional ids into ranks
     int64_t name_nbytes = 0, n_names = 0;
     // scanned accumulation (csv_scan_append_named_device, scan_api.inl): every decoded record of each packet.  scan_flag is the
@@ -122,8 +141,6 @@ struct ExtractState {
     // order, provisional ids) that csv_rank_names installs; rg_* the region table of csv_set_scan_regions.
     DBuf scan_flag, scan_excl, p_chrom, p_start, p_end, p_id, p_prim;
     DBuf rg_win_off, rg_win_start, rg_reg_off, rg_reg;
-    bool scanned = false;            // every packet of the accumulation was scanned
-    bool scan_aln = false;           // ... and asked for alignment rows
     int64_t n_pending = 0;
     int32_t rg_n_contigs = 0;        // 0: no region table
     double per_record[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // largest yield of a packet so far: signatures per type [0..4], pieces [5] per alignment record
@@ -538,7 +555,7 @@ extern "C" int csv_destroy(csv_ctx* c) {
         if (c->ev_side_fork[k]) cudaEventDestroy(c->ev_side_fork[k]);
         if (c->ev_side_join[k]) cudaEventDestroy(c->ev_side_join[k]);
     }
-    if (c->ex.h_counters) cudaFreeHost(c->ex.h_counters);
+    if (c->ex.h) cudaFreeHost(c->ex.h);
     for (cudaEvent_t e : c->ev_pool) cudaEventDestroy(e);
     if (c->h_counters) cudaFreeHost(c->h_counters);
     if (c->copy_stream) { cudaStreamSynchronize(c->copy_stream); cudaStreamDestroy(c->copy_stream); }
@@ -717,6 +734,17 @@ static int stage_group_offsets(csv_ctx* c, int slot, const int64_t* off, int64_t
     return CSV_OK;
 }
 
+// An upload replaced the device-resident inputs of one slot (an SV type, or the reads table): the rows no longer come from the
+// accumulation, which otherwise stays as it is
+static void inputs_replaced(csv_ctx* c, int slot) {
+    c->counts_valid = false;
+    c->ex.rec_valid = false;
+    c->ex.seq_valid = false;
+    c->ex.kind = PacketKind::PLAIN; c->ex.ranked = false;
+    c->ex.n_pending = 0;
+    c->up_checked[slot] = false;
+}
+
 static int upload_sigs_impl(csv_ctx* c, int t, const csv_sig_cols* h, const int64_t* contig_off, const UpSrc& src) {
     if (!c || t < 0 || t >= CSV_NTYPES || !h) return set_err(CSV_E_INVALID, "bad argument");
     if (h->n < 0 || h->n >= (1ll << 30)) return set_err(CSV_E_INVALID, "signature count %lld out of range", (long long)h->n);
@@ -724,12 +752,7 @@ static int upload_sigs_impl(csv_ctx* c, int t, const csv_sig_cols* h, const int6
     SigBuf& s = c->sig[t];
     s.n = h->n;
     s.has_c = h->c != nullptr;
-    c->counts_valid = false;
-    c->ex.rec_valid = false;
-    c->ex.seq_valid = false;
-    c->ex.named = false; c->ex.ranked = false;   // the rows no longer come from the named accumulation
-    c->ex.scanned = false; c->ex.n_pending = 0;
-    c->up_checked[t] = false;
+    inputs_replaced(c, t);
     if (h->n == 0) return CSV_OK;
     if ((!contig_off && !h->chrom) || !h->a || !h->b || !h->read_id) return set_err(CSV_E_INVALID, "null column");
     if ((t == CSV_INS || t == CSV_INV || t == CSV_TRA) && !h->c) return set_err(CSV_E_INVALID, "column c is required for INS/INV/TRA");
@@ -770,12 +793,7 @@ static int upload_reads_impl(csv_ctx* c, const csv_reads_cols* h, const int64_t*
     if (h->n < 0 || h->n >= (1ll << 31)) return set_err(CSV_E_INVALID, "read count out of range");
     CU(cudaSetDevice(c->device));
     c->n_reads = h->n;
-    c->counts_valid = false;
-    c->ex.rec_valid = false;
-    c->ex.seq_valid = false;
-    c->ex.named = false; c->ex.ranked = false;   // the rows no longer come from the named accumulation
-    c->ex.scanned = false; c->ex.n_pending = 0;
-    c->up_checked[CSV_NTYPES] = false;
+    inputs_replaced(c, CSV_NTYPES);
     if (h->n == 0) return CSV_OK;
     if ((!contig_off && !h->chrom) || !h->start || !h->end || !h->read_id || !h->is_primary) return set_err(CSV_E_INVALID, "null column");
     int rc;
@@ -841,7 +859,8 @@ static int upload_alignments_impl(csv_ctx* c, const csv_reads_cols* h, const UpS
     CU(cudaSetDevice(c->device));
     c->n_aln = h->n;
     c->counts_valid = false;
-    c->ex.scanned = false; c->ex.n_pending = 0;   // the table no longer comes from a scanned accumulation
+    if (kind_scanned(c->ex.kind)) c->ex.kind = PacketKind::NAMED;   // the table no longer comes from a scanned accumulation
+    c->ex.n_pending = 0;
     if (h->n == 0) return CSV_OK;
     if (!h->chrom || !h->start || !h->end || !h->read_id || !h->is_primary) return set_err(CSV_E_INVALID, "null column");
     if (src.device) {

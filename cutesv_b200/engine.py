@@ -399,342 +399,282 @@ class Engine(object):
         _lib.check(self.L.csv_result_device_ptrs(self.h, C.byref(a), C.byref(b), C.byref(c)))
         return a.value, b.value, c.value
 
+    def pin_packet(self, packed):
+        """Copy of an alignment packet in page-locked host memory (csv_host_alloc), so that csv_extract's H2D copies run at PCIe
+        speed and asynchronously.  The buffers are freed by close()."""
+        if not hasattr(self, "_pinned"):
+            self._pinned = []
+
+        def pin(a):
+            a = np.ascontiguousarray(a)
+            p = C.c_void_p()
+            _lib.check(self.L.csv_host_alloc(C.byref(p), C.c_size_t(max(a.nbytes, 1))))
+            self._pinned.append(p)
+            buf = (C.c_char * max(a.nbytes, 1)).from_address(p.value)
+            out = np.frombuffer(buf, dtype=a.dtype, count=a.size).reshape(a.shape)
+            out[...] = a
+            return out
+
+        out = {}
+        for k, v in packed.items():
+            if k == "sa":
+                out[k] = {kk: pin(np.asarray(vv, dtype=np.int32)) for kk, vv in v.items()}
+            elif k in ("cigar_off", "sa_off"):
+                out[k] = pin(np.asarray(v, dtype=np.int64))
+            elif k == "cigar":
+                out[k] = pin(np.asarray(v, dtype=np.uint32))
+            elif isinstance(v, np.ndarray) and v.dtype.kind in "iu" and k in ("chrom", "ref_start", "ref_end", "flag", "mapq", "query_len", "read_id"):
+                out[k] = pin(np.asarray(v, dtype=np.int32))
+            else:
+                out[k] = v
+        return out
+
+    def extract(self, packed, append=False, stream=None):
+        """csv_extract on a packing.pack_alignments() packet.  The extracted signatures and reads rows
+        stay device-resident as the inputs of cluster_device(); returns dict(counts, n_rows).
+        append=True (csv_extract_append): this packet's output is appended to what earlier packets left on the device;
+        counts / n_rows are the totals so far and `first` holds the totals before this packet.
+        A packet whose arrays expose __cuda_array_interface__ (torch CUDA tensors; see _abi.device_packet) goes through
+        csv_extract*_device in the order of `stream` (see _producer_stream), and with seq_off / seq4 (BAM's packed bases) the INS
+        sequences are built on the device (fetch_ins_seqs, ins_seq_tensors).  Device and host packets may be mixed in one
+        append accumulation.  A device packet with names / name_off (the records' read names as bytes, instead of read_id) goes
+        through csv_extract*_named_device: every packet of the accumulation then carries names, and rank_names() turns the
+        provisional ids (record indices) into name ranks."""
+        counts = (C.c_int64 * _abi.CSV_NTYPES)()
+        n_rows = C.c_int64(0)
+        d = _abi.device_packet(packed, self.device)
+        if d is not None:
+            rc_, cig_p, n_cig, sa_, seq = d
+            st = self._producer_stream(stream, [packed])
+            seq_p = C.byref(seq) if seq is not None else None
+            if d.names is not None:
+                fn = self.L.csv_extract_append_named_device if append else self.L.csv_extract_named_device
+                _lib.check(fn(self.h, C.byref(rc_), cig_p, C.c_int64(n_cig), C.byref(sa_), seq_p, C.byref(d.names), C.c_void_p(st or None), counts,
+                              C.byref(n_rows)))
+            else:
+                fn = self.L.csv_extract_append_device if append else self.L.csv_extract_device
+                _lib.check(fn(self.h, C.byref(rc_), cig_p, C.c_int64(n_cig), C.byref(sa_), seq_p, C.c_void_p(st or None), counts, C.byref(n_rows)))
+        else:
+            n = len(packed["chrom"])
+            keep = [np.ascontiguousarray(packed[k], dtype=np.int32) for k in ("chrom", "ref_start", "ref_end", "flag", "mapq", "query_len", "read_id")]
+            co = np.ascontiguousarray(packed["cigar_off"], dtype=np.int64)
+            so = np.ascontiguousarray(packed["sa_off"], dtype=np.int64)
+            rc_ = _abi.csv_read_cols(n, *[_abi.ptr(k) for k in keep], co.ctypes.data_as(C.POINTER(C.c_int64)), so.ctypes.data_as(C.POINTER(C.c_int64)))
+            sa = {k: np.ascontiguousarray(v, dtype=np.int32) for k, v in packed["sa"].items()}
+            sa_ = _abi.csv_sa_cols(len(sa["chrom"]), *[_abi.ptr(sa[k]) for k in ("chrom", "pos0", "strand", "mapq", "first_clip", "last_clip", "ref_span")])
+            cig = np.ascontiguousarray(packed["cigar"], dtype=np.uint32)
+            fn = self.L.csv_extract_append if append else self.L.csv_extract
+            _lib.check(fn(self.h, C.byref(rc_), cig.ctypes.data_as(C.POINTER(C.c_uint32)), C.c_int64(len(cig)), C.byref(sa_), counts, C.byref(n_rows)))
+        return self._extracted(counts, n_rows, append)
+
+    def _extracted(self, counts, n_rows, append):
+        """Bookkeeping after an extraction call and extract()'s result.  `first*`: the totals before this packet, which the
+        mirrors still hold when the packet joined the open accumulation."""
+        joined = append and getattr(self, "_ex_appending", False)
+        first = self._ex_counts if joined else [0] * _abi.CSV_NTYPES
+        first_rows = self._ex_rows if joined else 0
+        first_pieces = self._ex_pieces if joined else 0
+        self._ex_counts = [int(x) for x in counts]
+        self._ex_rows = int(n_rows.value)
+        self._dev_rows = self._ex_counts + [self._ex_rows]
+        self._ex_appending = bool(append)
+        npz = C.c_int64(0)
+        _lib.check(self.L.csv_fetch_pieces(self.h, C.c_int64(0), None, C.byref(npz)))
+        self._ex_pieces = int(npz.value)
+        return dict(counts={name: int(counts[t]) for t, name in enumerate(_abi.TYPE_NAMES)}, n_rows=int(n_rows.value),
+                    first={name: first[t] for t, name in enumerate(_abi.TYPE_NAMES)}, first_rows=first_rows, first_pieces=first_pieces,
+                    n_pieces=self._ex_pieces)
+
+    def set_scan_regions(self, tasks, bed, chrom_id):
+        """Region table of the following scan() calls (csv_set_scan_regions) from cli.task_windows' tasks, cli.load_bed's region lists
+        and the contig ids; bed None clears it.  With a table, scan() extracts only the records the CLI keeps with -include_bed."""
+        n, win_off, win_start, reg_off, reg = _abi.scan_regions(tasks, bed, chrom_id)
+        if n == 0:
+            _lib.check(self.L.csv_set_scan_regions(self.h, C.c_int32(0), None, None, None, None))
+            return
+        _lib.check(self.L.csv_set_scan_regions(self.h, C.c_int32(n), win_off.ctypes.data_as(C.POINTER(C.c_int64)),
+                                               win_start.ctypes.data_as(C.POINTER(C.c_double)), reg_off.ctypes.data_as(C.POINTER(C.c_int64)),
+                                               reg.ctypes.data_as(C.POINTER(C.c_int64))))
+
+    def fetch_alignments(self):
+        """D2H of csv_cluster's alignment table (upload_alignments, or installed by rank_names after scan(..., alignments=True)):
+        dict(chrom, start, end, read_id, is_primary) in the table's order, or None when there is none."""
+        n = C.c_int64(0)
+        rc = self.L.csv_fetch_alignments(self.h, C.c_int64(0), None, None, None, None, None, C.byref(n))
+        if rc != _abi.CSV_E_CAPACITY:   # the size probe
+            _lib.check(rc)
+        if n.value == 0:
+            return None
+        k = n.value
+        cols = {c: np.zeros(k, dtype=np.int32) for c in ("chrom", "start", "end", "read_id")}
+        cols["is_primary"] = np.zeros(k, dtype=np.uint8)
+        _lib.check(self.L.csv_fetch_alignments(self.h, C.c_int64(k), *[_abi.ptr(cols[c]) for c in ("chrom", "start", "end", "read_id")],
+                                               cols["is_primary"].ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(n)))
+        return cols
+
+    def scan(self, packet, alignments=False, stream=None):
+        """Appends every decoded record of a BAM packet (csv_scan_append_named_device): a torch CUDA packet with names / name_off and
+        no read_id (_abi.scan_packet).  The library drops what the reference's single_pipe drops (no CIGAR, contig < 0, flag 256 or
+        272, outside the set_scan_regions table) and extracts the rest in place; alignments=True also keeps every record with a CIGAR
+        and a contig as a row of the TRA genotyper's alignment table, which rank_names() installs.  Record numbers (provisional ids,
+        name_rank_tensor, fetch_records, INS pieces) count all scanned records.  Returns extract()'s dict plus n_aln_rows."""
+        d = _abi.scan_packet(packet, self.device)
+        rc_, cig_p, n_cig, sa_, seq = d
+        counts = (C.c_int64 * _abi.CSV_NTYPES)()
+        n_rows, n_aln = C.c_int64(0), C.c_int64(0)
+        st = self._producer_stream(stream, [packet])
+        _lib.check(self.L.csv_scan_append_named_device(self.h, C.byref(rc_), cig_p, C.c_int64(n_cig), C.byref(sa_),
+                                                       C.byref(seq) if seq is not None else None, C.byref(d.names), int(bool(alignments)),
+                                                       C.c_void_p(st or None), counts, C.byref(n_rows), C.byref(n_aln)))
+        out = self._extracted(counts, n_rows, True)
+        out["n_aln_rows"] = int(n_aln.value)
+        return out
+
+    def fetch_ins_seqs(self, rows):
+        """Sequence strings of INS rows `rows` from the device-built arena (csv_fetch_ins_seqs: one gather, one D2H copy).
+        Needs an accumulation whose packets all were device packets with bases; CuteSVError CSV_E_STATE otherwise."""
+        rows = np.ascontiguousarray(rows, dtype=np.int64).reshape(-1)
+        whole, o = self._fetch_arena(self.L.csv_fetch_ins_seqs, rows.ctypes.data_as(C.POINTER(C.c_int64)), len(rows), 512 * len(rows) + 4096)
+        whole = whole.decode("ascii")
+        return [whole[o[i]:o[i + 1]] for i in range(len(rows))]
+
+    def _fetch_arena(self, fn, rows, n, cap):
+        """(bytes, offsets list) of csv_fetch_ins_seqs / csv_fetch_names on n rows: first with `cap` bytes of room, then with the
+        room a CSV_E_CAPACITY reports."""
+        off = np.zeros(n + 1, dtype=np.int64)
+        while True:
+            out = np.zeros(max(cap, 1), dtype=np.uint8)
+            rc = fn(self.h, rows, C.c_int64(n), out.ctypes.data_as(C.POINTER(C.c_uint8)), C.c_int64(cap), off.ctypes.data_as(C.POINTER(C.c_int64)))
+            if rc != _abi.CSV_E_CAPACITY:
+                break
+            cap = int(off[n])
+        _lib.check(rc)
+        return out[:int(off[n])].tobytes(), off.tolist()
+
+    def ins_seq_tensors(self):
+        """Zero-copy torch views of the device-built INS sequence arena: (bytes uint8, start int64 [n_rows], length int32 [n_rows]);
+        row k's string is bytes[start[k]:start[k] + length[k]].  Valid until the next extract, upload or swap_ins_rows on this
+        engine, so clone() whatever you keep."""
+        import torch
+        b, s, ln, nr = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_int64(0)
+        _lib.check(self.L.csv_ins_seq_device_ptrs(self.h, C.byref(b), C.byref(s), C.byref(ln), C.byref(nr)))
+        dev = torch.device("cuda", self.device)
+        n = nr.value
+        start = torch.as_tensor(_DeviceView(s.value, (n,), "<i8"), device=dev)
+        length = torch.as_tensor(_DeviceView(ln.value, (n,)), device=dev)
+        nbytes = int((start + length.to(torch.int64)).max()) if n else 0
+        return torch.as_tensor(_DeviceView(b.value, (nbytes,), "|u1"), device=dev), start, length
+
+    def rank_names(self):
+        """Ranks the read names of a named accumulation on the device (csv_rank_names): every signature's and reads row's read id
+        becomes the dense rank of its name in byte (for UTF-8: Python str) order.  After scan(..., alignments=True) it also installs
+        the scanned alignment rows, ids as ranks and sorted by contig, as the TRA genotyper's table.  Returns the number of distinct
+        names."""
+        nd = C.c_int64(0)
+        _lib.check(self.L.csv_rank_names(self.h, C.byref(nd)))
+        return int(nd.value)
+
+    def fetch_names(self, ranks):
+        """Read names (str) of name ranks `ranks` (any order, repeats allowed) after rank_names (csv_fetch_names)."""
+        ranks = np.ascontiguousarray(ranks, dtype=np.int32).reshape(-1)
+        raw, o = self._fetch_arena(self.L.csv_fetch_names, _abi.ptr(ranks), len(ranks), 64 * len(ranks) + 256)
+        return [raw[o[i]:o[i + 1]].decode("utf-8") for i in range(len(ranks))]
+
+    def name_rank_tensor(self):
+        """Zero-copy torch view (int32, one entry per record of the accumulation) of the table record index -> name rank that
+        rank_names built, e.g. to turn a caller-built alignment table's provisional ids into ranks with one gather.  Valid until the
+        next extract or extract_reset on this engine, so clone() what you keep."""
+        import torch
+        p, nr = C.c_void_p(), C.c_int64(0)
+        _lib.check(self.L.csv_name_ranks_device_ptr(self.h, C.byref(p), C.byref(nr)))
+        return torch.as_tensor(_DeviceView(p.value, (nr.value,)), device=torch.device("cuda", self.device))
+
+    def order_ins_ties(self):
+        """Puts INS rows that tie on (contig, int(pos), len, read) into the order of their device-built sequences (csv_order_ins_ties):
+        what ins_tie_swaps + swap_ins_rows do on the host.  The read ids must be ranks (rank_names or remap_read_ids first).  Returns
+        the number of rows whose content moved."""
+        nm = C.c_int64(0)
+        _lib.check(self.L.csv_order_ins_ties(self.h, C.byref(nm)))
+        return int(nm.value)
+
+    def extract_skipped(self):
+        """Records whose split-read analysis was skipped (more than 64 qualifying segments, only with max_split_parts -1)."""
+        return int(self.L.csv_extract_skipped(self.h))
+
+    def extract_reset(self):
+        _lib.check(self.L.csv_extract_reset(self.h))
+        self._ex_counts = [0] * _abi.CSV_NTYPES
+        self._ex_rows = 0
+        self._ex_pieces = 0
+        self._ex_appending = False
+        self._dev_rows = [0] * (_abi.CSV_NTYPES + 1)
+
+    def fetch_ins_pieces(self, first_sig, n_sig, first_piece, n_piece):
+        """Piece descriptors of INS signatures [first_sig, first_sig + n_sig) and pieces [first_piece, first_piece + n_piece):
+        what the host needs to rebuild the sequences of the rows ONE packet appended.  piece_off is re-based to the slice."""
+        po = np.zeros(max(n_sig, 1), dtype=np.int32)
+        pc = np.zeros(max(n_sig, 1), dtype=np.int32)
+        if n_sig:
+            _lib.check(self.L.csv_fetch_sigs_range(self.h, _abi.CSV_INS, C.c_int64(first_sig), C.c_int64(n_sig), None, None, None, None, None,
+                                                   _abi.ptr(po), _abi.ptr(pc)))
+        pieces = np.zeros((max(n_piece, 1), 4), dtype=np.int32)
+        if n_piece:
+            _lib.check(self.L.csv_fetch_pieces_range(self.h, C.c_int64(first_piece), C.c_int64(n_piece), _abi.ptr(pieces)))
+        return po[:n_sig] - first_piece, pc[:n_sig], pieces[:n_piece]
+
+    def fetch_sig_cols(self, name, cols=("chrom", "a", "b", "read_id", "c")):
+        """D2H of whole columns of the device-resident signatures of one type."""
+        t = _abi.TYPE_IDS[name]
+        k = self._ex_counts[t]
+        out = {c: (np.zeros(max(k, 1), dtype=np.int32) if c in cols else None) for c in ("chrom", "a", "b", "read_id", "c")}
+        if k:
+            _lib.check(self.L.csv_fetch_sigs_range(self.h, t, C.c_int64(0), C.c_int64(k), *[(_abi.ptr(out[c]) if out[c] is not None else None)
+                                                                                              for c in ("chrom", "a", "b", "read_id", "c")], None, None))
+        return {c: (v[:k] if v is not None else None) for c, v in out.items()}
+
+    def fetch_read_rows(self):
+        """D2H of the device-resident reads table (reads_info_list rows, cuteSV:729-733)."""
+        nr = self._ex_rows
+        rows = {k: np.zeros(max(nr, 1), dtype=np.int32) for k in ("chrom", "start", "end", "read_id")}
+        prim = np.zeros(max(nr, 1), dtype=np.uint8)
+        _lib.check(self.L.csv_fetch_read_rows(self.h, C.c_int64(max(nr, 1)), _abi.ptr(rows["chrom"]), _abi.ptr(rows["start"]), _abi.ptr(rows["end"]),
+                                              _abi.ptr(rows["read_id"]), prim.ctypes.data_as(C.POINTER(C.c_uint8))))
+        rows = {k: v[:nr] for k, v in rows.items()}
+        rows["is_primary"] = prim[:nr]
+        return rows
+
+    def remap_read_ids(self, rank):
+        rank = np.ascontiguousarray(rank, dtype=np.int32)
+        _lib.check(self.L.csv_remap_read_ids(self.h, _abi.ptr(rank), C.c_int64(len(rank))))
+
+    def swap_ins_rows(self, pairs):
+        pairs = np.ascontiguousarray(pairs, dtype=np.int64).reshape(-1, 2)
+        if len(pairs):
+            _lib.check(self.L.csv_swap_ins_rows(self.h, pairs.ctypes.data_as(C.POINTER(C.c_int64)), C.c_int64(len(pairs))))
+
+    def fetch_extracted(self):
+        """D2H of everything csv_extract produced (parity tests / host ALT strings)."""
+        sigs = {}
+        poff = pcnt = None
+        for t, name in enumerate(_abi.TYPE_NAMES):
+            k = self._ex_counts[t]
+            cols = {c: np.zeros(max(k, 1), dtype=np.int32) for c in ("chrom", "a", "b", "read_id", "c")}
+            po = np.zeros(max(k, 1), dtype=np.int32)
+            pc = np.zeros(max(k, 1), dtype=np.int32)
+            _lib.check(self.L.csv_fetch_sigs(self.h, t, C.c_int64(max(k, 1)), _abi.ptr(cols["chrom"]), _abi.ptr(cols["a"]), _abi.ptr(cols["b"]),
+                                             _abi.ptr(cols["read_id"]), _abi.ptr(cols["c"]), _abi.ptr(po), _abi.ptr(pc)))
+            sigs[name] = {c: v[:k] for c, v in cols.items()}
+            if name == "INS":
+                poff, pcnt = po[:k], pc[:k]
+        npz = C.c_int64(0)
+        _lib.check(self.L.csv_fetch_pieces(self.h, C.c_int64(0), None, C.byref(npz)))
+        pieces = np.zeros((max(npz.value, 1), 4), dtype=np.int32)
+        _lib.check(self.L.csv_fetch_pieces(self.h, C.c_int64(len(pieces)), _abi.ptr(pieces), C.byref(npz)))
+        return dict(sigs=sigs, piece_off=poff, piece_cnt=pcnt, pieces=pieces[:npz.value], rows=self.fetch_read_rows())
+
 
 class _DeviceView(object):
     """__cuda_array_interface__ of an array the library owns (torch.as_tensor makes a view of it, no copy); int32 by default."""
 
     def __init__(self, ptr, shape, typestr="<i4"):
         self.__cuda_array_interface__ = {"shape": tuple(shape), "typestr": typestr, "data": (int(ptr or 0), False), "version": 2}
-
-
-def _pin_packet_method(self, packed):
-    """Copy of an alignment packet in page-locked host memory (csv_host_alloc), so that csv_extract's H2D copies run at PCIe
-    speed and asynchronously.  The buffers are freed by close()."""
-    if not hasattr(self, "_pinned"):
-        self._pinned = []
-
-    def pin(a):
-        a = np.ascontiguousarray(a)
-        p = C.c_void_p()
-        _lib.check(self.L.csv_host_alloc(C.byref(p), C.c_size_t(max(a.nbytes, 1))))
-        self._pinned.append(p)
-        buf = (C.c_char * max(a.nbytes, 1)).from_address(p.value)
-        out = np.frombuffer(buf, dtype=a.dtype, count=a.size).reshape(a.shape)
-        out[...] = a
-        return out
-
-    out = {}
-    for k, v in packed.items():
-        if k == "sa":
-            out[k] = {kk: pin(np.asarray(vv, dtype=np.int32)) for kk, vv in v.items()}
-        elif k in ("cigar_off", "sa_off"):
-            out[k] = pin(np.asarray(v, dtype=np.int64))
-        elif k == "cigar":
-            out[k] = pin(np.asarray(v, dtype=np.uint32))
-        elif isinstance(v, np.ndarray) and v.dtype.kind in "iu" and k in ("chrom", "ref_start", "ref_end", "flag", "mapq", "query_len", "read_id"):
-            out[k] = pin(np.asarray(v, dtype=np.int32))
-        else:
-            out[k] = v
-    return out
-
-
-def _extract_method(self, packed, append=False, stream=None):
-    """csv_extract on a packing.pack_alignments() packet.  The extracted signatures and reads rows
-    stay device-resident as the inputs of cluster_device(); returns dict(counts, n_rows).
-    append=True (csv_extract_append): this packet's output is appended to what earlier packets left on the device;
-    counts / n_rows are the totals so far and `first` holds the totals before this packet.
-    A packet whose arrays expose __cuda_array_interface__ (torch CUDA tensors; see _abi.device_packet) goes through
-    csv_extract*_device in the order of `stream` (see _producer_stream), and with seq_off / seq4 (BAM's packed bases) the INS
-    sequences are built on the device (fetch_ins_seqs, ins_seq_tensors).  Device and host packets may be mixed in one
-    append accumulation.  A device packet with names / name_off (the records' read names as bytes, instead of read_id) goes
-    through csv_extract*_named_device: every packet of the accumulation then carries names, and rank_names() turns the
-    provisional ids (record indices) into name ranks."""
-    counts = (C.c_int64 * _abi.CSV_NTYPES)()
-    n_rows = C.c_int64(0)
-    first = list(getattr(self, "_ex_counts", [0] * _abi.CSV_NTYPES)) if (append and getattr(self, "_ex_appending", False)) else [0] * _abi.CSV_NTYPES
-    first_rows = getattr(self, "_ex_rows", 0) if (append and getattr(self, "_ex_appending", False)) else 0
-    first_pieces = getattr(self, "_ex_pieces", 0) if (append and getattr(self, "_ex_appending", False)) else 0
-    d = _abi.device_packet(packed, self.device)
-    if d is not None:
-        rc_, cig_p, n_cig, sa_, seq = d
-        st = self._producer_stream(stream, [packed])
-        seq_p = C.byref(seq) if seq is not None else None
-        if d.names is not None:
-            fn = self.L.csv_extract_append_named_device if append else self.L.csv_extract_named_device
-            _lib.check(fn(self.h, C.byref(rc_), cig_p, C.c_int64(n_cig), C.byref(sa_), seq_p, C.byref(d.names), C.c_void_p(st or None), counts,
-                          C.byref(n_rows)))
-        else:
-            fn = self.L.csv_extract_append_device if append else self.L.csv_extract_device
-            _lib.check(fn(self.h, C.byref(rc_), cig_p, C.c_int64(n_cig), C.byref(sa_), seq_p, C.c_void_p(st or None), counts, C.byref(n_rows)))
-    else:
-        n = len(packed["chrom"])
-        keep = [np.ascontiguousarray(packed[k], dtype=np.int32) for k in ("chrom", "ref_start", "ref_end", "flag", "mapq", "query_len", "read_id")]
-        co = np.ascontiguousarray(packed["cigar_off"], dtype=np.int64)
-        so = np.ascontiguousarray(packed["sa_off"], dtype=np.int64)
-        rc_ = _abi.csv_read_cols(n, *[_abi.ptr(k) for k in keep], co.ctypes.data_as(C.POINTER(C.c_int64)), so.ctypes.data_as(C.POINTER(C.c_int64)))
-        sa = {k: np.ascontiguousarray(v, dtype=np.int32) for k, v in packed["sa"].items()}
-        sa_ = _abi.csv_sa_cols(len(sa["chrom"]), *[_abi.ptr(sa[k]) for k in ("chrom", "pos0", "strand", "mapq", "first_clip", "last_clip", "ref_span")])
-        cig = np.ascontiguousarray(packed["cigar"], dtype=np.uint32)
-        fn = self.L.csv_extract_append if append else self.L.csv_extract
-        _lib.check(fn(self.h, C.byref(rc_), cig.ctypes.data_as(C.POINTER(C.c_uint32)), C.c_int64(len(cig)), C.byref(sa_), counts, C.byref(n_rows)))
-    return _extracted(self, counts, n_rows, append, first, first_rows, first_pieces)
-
-
-def _extracted(self, counts, n_rows, append, first, first_rows, first_pieces):
-    """Bookkeeping after an extraction call and extract()'s result."""
-    self._ex_counts = [int(x) for x in counts]
-    self._ex_rows = int(n_rows.value)
-    self._dev_rows = self._ex_counts + [self._ex_rows]
-    self._ex_appending = bool(append)
-    npz = C.c_int64(0)
-    _lib.check(self.L.csv_fetch_pieces(self.h, C.c_int64(0), None, C.byref(npz)))
-    self._ex_pieces = int(npz.value)
-    return dict(counts={name: int(counts[t]) for t, name in enumerate(_abi.TYPE_NAMES)}, n_rows=int(n_rows.value),
-                first={name: first[t] for t, name in enumerate(_abi.TYPE_NAMES)}, first_rows=first_rows, first_pieces=first_pieces,
-                n_pieces=self._ex_pieces)
-
-
-def _set_scan_regions_method(self, tasks, bed, chrom_id):
-    """Region table of the following scan() calls (csv_set_scan_regions) from cli.task_windows' tasks, cli.load_bed's region lists
-    and the contig ids; bed None clears it.  With a table, scan() extracts only the records the CLI keeps with -include_bed."""
-    n, win_off, win_start, reg_off, reg = _abi.scan_regions(tasks, bed, chrom_id)
-    if n == 0:
-        _lib.check(self.L.csv_set_scan_regions(self.h, C.c_int32(0), None, None, None, None))
-        return
-    _lib.check(self.L.csv_set_scan_regions(self.h, C.c_int32(n), win_off.ctypes.data_as(C.POINTER(C.c_int64)),
-                                           win_start.ctypes.data_as(C.POINTER(C.c_double)), reg_off.ctypes.data_as(C.POINTER(C.c_int64)),
-                                           reg.ctypes.data_as(C.POINTER(C.c_int64))))
-
-
-def _fetch_alignments_method(self):
-    """D2H of csv_cluster's alignment table (upload_alignments, or installed by rank_names after scan(..., alignments=True)):
-    dict(chrom, start, end, read_id, is_primary) in the table's order, or None when there is none."""
-    n = C.c_int64(0)
-    rc = self.L.csv_fetch_alignments(self.h, C.c_int64(0), None, None, None, None, None, C.byref(n))
-    if rc != _abi.CSV_E_CAPACITY:   # the size probe
-        _lib.check(rc)
-    if n.value == 0:
-        return None
-    k = n.value
-    cols = {c: np.zeros(k, dtype=np.int32) for c in ("chrom", "start", "end", "read_id")}
-    cols["is_primary"] = np.zeros(k, dtype=np.uint8)
-    _lib.check(self.L.csv_fetch_alignments(self.h, C.c_int64(k), *[_abi.ptr(cols[c]) for c in ("chrom", "start", "end", "read_id")],
-                                           cols["is_primary"].ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(n)))
-    return cols
-
-
-def _scan_method(self, packet, alignments=False, stream=None):
-    """Appends every decoded record of a BAM packet (csv_scan_append_named_device): a torch CUDA packet with names / name_off and
-    no read_id (_abi.scan_packet).  The library drops what the reference's single_pipe drops (no CIGAR, contig < 0, flag 256 or
-    272, outside the set_scan_regions table) and extracts the rest in place; alignments=True also keeps every record with a CIGAR
-    and a contig as a row of the TRA genotyper's alignment table, which rank_names() installs.  Record numbers (provisional ids,
-    name_rank_tensor, fetch_records, INS pieces) count all scanned records.  Returns extract()'s dict plus n_aln_rows."""
-    d = _abi.scan_packet(packet, self.device)
-    rc_, cig_p, n_cig, sa_, seq = d
-    appending = getattr(self, "_ex_appending", False)
-    first = list(getattr(self, "_ex_counts", [0] * _abi.CSV_NTYPES)) if appending else [0] * _abi.CSV_NTYPES
-    first_rows = getattr(self, "_ex_rows", 0) if appending else 0
-    first_pieces = getattr(self, "_ex_pieces", 0) if appending else 0
-    counts = (C.c_int64 * _abi.CSV_NTYPES)()
-    n_rows, n_aln = C.c_int64(0), C.c_int64(0)
-    st = self._producer_stream(stream, [packet])
-    _lib.check(self.L.csv_scan_append_named_device(self.h, C.byref(rc_), cig_p, C.c_int64(n_cig), C.byref(sa_),
-                                                   C.byref(seq) if seq is not None else None, C.byref(d.names), int(bool(alignments)),
-                                                   C.c_void_p(st or None), counts, C.byref(n_rows), C.byref(n_aln)))
-    out = _extracted(self, counts, n_rows, True, first, first_rows, first_pieces)
-    out["n_aln_rows"] = int(n_aln.value)
-    return out
-
-
-def _fetch_ins_seqs_method(self, rows):
-    """Sequence strings of INS rows `rows` from the device-built arena (csv_fetch_ins_seqs: one gather, one D2H copy).
-    Needs an accumulation whose packets all were device packets with bases; CuteSVError CSV_E_STATE otherwise."""
-    rows = np.ascontiguousarray(rows, dtype=np.int64).reshape(-1)
-    n = len(rows)
-    off = np.zeros(n + 1, dtype=np.int64)
-    cap = 512 * n + 4096
-    while True:
-        out = np.zeros(max(cap, 1), dtype=np.uint8)
-        rc = self.L.csv_fetch_ins_seqs(self.h, rows.ctypes.data_as(C.POINTER(C.c_int64)), C.c_int64(n), out.ctypes.data_as(C.POINTER(C.c_uint8)),
-                                       C.c_int64(cap), off.ctypes.data_as(C.POINTER(C.c_int64)))
-        if rc != _abi.CSV_E_CAPACITY:
-            break
-        cap = int(off[n])
-    _lib.check(rc)
-    whole = out[:int(off[n])].tobytes().decode("ascii")
-    o = off.tolist()
-    return [whole[o[i]:o[i + 1]] for i in range(n)]
-
-
-def _ins_seq_tensors_method(self):
-    """Zero-copy torch views of the device-built INS sequence arena: (bytes uint8, start int64 [n_rows], length int32 [n_rows]);
-    row k's string is bytes[start[k]:start[k] + length[k]].  Valid until the next extract, upload or swap_ins_rows on this
-    engine, so clone() whatever you keep."""
-    import torch
-    b, s, ln, nr = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_int64(0)
-    _lib.check(self.L.csv_ins_seq_device_ptrs(self.h, C.byref(b), C.byref(s), C.byref(ln), C.byref(nr)))
-    dev = torch.device("cuda", self.device)
-    n = nr.value
-    start = torch.as_tensor(_DeviceView(s.value, (n,), "<i8"), device=dev)
-    length = torch.as_tensor(_DeviceView(ln.value, (n,)), device=dev)
-    nbytes = int((start + length.to(torch.int64)).max()) if n else 0
-    return torch.as_tensor(_DeviceView(b.value, (nbytes,), "|u1"), device=dev), start, length
-
-
-def _rank_names_method(self):
-    """Ranks the read names of a named accumulation on the device (csv_rank_names): every signature's and reads row's read id
-    becomes the dense rank of its name in byte (for UTF-8: Python str) order.  After scan(..., alignments=True) it also installs
-    the scanned alignment rows, ids as ranks and sorted by contig, as the TRA genotyper's table.  Returns the number of distinct
-    names."""
-    nd = C.c_int64(0)
-    _lib.check(self.L.csv_rank_names(self.h, C.byref(nd)))
-    return int(nd.value)
-
-
-def _fetch_names_method(self, ranks):
-    """Read names (str) of name ranks `ranks` (any order, repeats allowed) after rank_names (csv_fetch_names)."""
-    ranks = np.ascontiguousarray(ranks, dtype=np.int32).reshape(-1)
-    n = len(ranks)
-    off = np.zeros(n + 1, dtype=np.int64)
-    cap = 64 * n + 256
-    while True:
-        out = np.zeros(max(cap, 1), dtype=np.uint8)
-        rc = self.L.csv_fetch_names(self.h, _abi.ptr(ranks), C.c_int64(n), out.ctypes.data_as(C.POINTER(C.c_uint8)), C.c_int64(cap),
-                                    off.ctypes.data_as(C.POINTER(C.c_int64)))
-        if rc != _abi.CSV_E_CAPACITY:
-            break
-        cap = int(off[n])
-    _lib.check(rc)
-    raw = out[:int(off[n])].tobytes()
-    o = off.tolist()
-    return [raw[o[i]:o[i + 1]].decode("utf-8") for i in range(n)]
-
-
-def _name_rank_tensor_method(self):
-    """Zero-copy torch view (int32, one entry per record of the accumulation) of the table record index -> name rank that
-    rank_names built, e.g. to turn a caller-built alignment table's provisional ids into ranks with one gather.  Valid until the
-    next extract or extract_reset on this engine, so clone() what you keep."""
-    import torch
-    p, nr = C.c_void_p(), C.c_int64(0)
-    _lib.check(self.L.csv_name_ranks_device_ptr(self.h, C.byref(p), C.byref(nr)))
-    return torch.as_tensor(_DeviceView(p.value, (nr.value,)), device=torch.device("cuda", self.device))
-
-
-def _order_ins_ties_method(self):
-    """Puts INS rows that tie on (contig, int(pos), len, read) into the order of their device-built sequences (csv_order_ins_ties):
-    what ins_tie_swaps + swap_ins_rows do on the host.  The read ids must be ranks (rank_names or remap_read_ids first).  Returns
-    the number of rows whose content moved."""
-    nm = C.c_int64(0)
-    _lib.check(self.L.csv_order_ins_ties(self.h, C.byref(nm)))
-    return int(nm.value)
-
-
-def _extract_skipped_method(self):
-    """Records whose split-read analysis was skipped (more than 64 qualifying segments, only with max_split_parts -1)."""
-    return int(self.L.csv_extract_skipped(self.h))
-
-
-def _extract_reset_method(self):
-    _lib.check(self.L.csv_extract_reset(self.h))
-    self._ex_counts = [0] * _abi.CSV_NTYPES
-    self._ex_rows = 0
-    self._ex_pieces = 0
-    self._ex_appending = False
-    self._dev_rows = [0] * (_abi.CSV_NTYPES + 1)
-
-
-def _fetch_ins_pieces_method(self, first_sig, n_sig, first_piece, n_piece):
-    """Piece descriptors of INS signatures [first_sig, first_sig + n_sig) and pieces [first_piece, first_piece + n_piece):
-    what the host needs to rebuild the sequences of the rows ONE packet appended.  piece_off is re-based to the slice."""
-    po = np.zeros(max(n_sig, 1), dtype=np.int32)
-    pc = np.zeros(max(n_sig, 1), dtype=np.int32)
-    if n_sig:
-        _lib.check(self.L.csv_fetch_sigs_range(self.h, _abi.CSV_INS, C.c_int64(first_sig), C.c_int64(n_sig), None, None, None, None, None,
-                                               _abi.ptr(po), _abi.ptr(pc)))
-    pieces = np.zeros((max(n_piece, 1), 4), dtype=np.int32)
-    if n_piece:
-        _lib.check(self.L.csv_fetch_pieces_range(self.h, C.c_int64(first_piece), C.c_int64(n_piece), _abi.ptr(pieces)))
-    return po[:n_sig] - first_piece, pc[:n_sig], pieces[:n_piece]
-
-
-def _fetch_sig_cols_method(self, name, cols=("chrom", "a", "b", "read_id", "c")):
-    """D2H of whole columns of the device-resident signatures of one type."""
-    t = _abi.TYPE_IDS[name]
-    k = self._ex_counts[t]
-    out = {c: (np.zeros(max(k, 1), dtype=np.int32) if c in cols else None) for c in ("chrom", "a", "b", "read_id", "c")}
-    if k:
-        _lib.check(self.L.csv_fetch_sigs_range(self.h, t, C.c_int64(0), C.c_int64(k), *[(_abi.ptr(out[c]) if out[c] is not None else None)
-                                                                                          for c in ("chrom", "a", "b", "read_id", "c")], None, None))
-    return {c: (v[:k] if v is not None else None) for c, v in out.items()}
-
-
-def _fetch_read_rows_method(self):
-    """D2H of the device-resident reads table (reads_info_list rows, cuteSV:729-733)."""
-    nr = self._ex_rows
-    rows = {k: np.zeros(max(nr, 1), dtype=np.int32) for k in ("chrom", "start", "end", "read_id")}
-    prim = np.zeros(max(nr, 1), dtype=np.uint8)
-    _lib.check(self.L.csv_fetch_read_rows(self.h, C.c_int64(max(nr, 1)), _abi.ptr(rows["chrom"]), _abi.ptr(rows["start"]), _abi.ptr(rows["end"]),
-                                          _abi.ptr(rows["read_id"]), prim.ctypes.data_as(C.POINTER(C.c_uint8))))
-    rows = {k: v[:nr] for k, v in rows.items()}
-    rows["is_primary"] = prim[:nr]
-    return rows
-
-
-def _remap_read_ids_method(self, rank):
-    rank = np.ascontiguousarray(rank, dtype=np.int32)
-    _lib.check(self.L.csv_remap_read_ids(self.h, _abi.ptr(rank), C.c_int64(len(rank))))
-
-
-def _swap_ins_rows_method(self, pairs):
-    pairs = np.ascontiguousarray(pairs, dtype=np.int64).reshape(-1, 2)
-    if len(pairs):
-        _lib.check(self.L.csv_swap_ins_rows(self.h, pairs.ctypes.data_as(C.POINTER(C.c_int64)), C.c_int64(len(pairs))))
-
-
-def _fetch_extracted_method(self):
-    """D2H of everything csv_extract produced (parity tests / host ALT strings)."""
-    sigs = {}
-    poff = pcnt = None
-    for t, name in enumerate(_abi.TYPE_NAMES):
-        k = self._ex_counts[t]
-        cols = {c: np.zeros(max(k, 1), dtype=np.int32) for c in ("chrom", "a", "b", "read_id", "c")}
-        po = np.zeros(max(k, 1), dtype=np.int32)
-        pc = np.zeros(max(k, 1), dtype=np.int32)
-        _lib.check(self.L.csv_fetch_sigs(self.h, t, C.c_int64(max(k, 1)), _abi.ptr(cols["chrom"]), _abi.ptr(cols["a"]), _abi.ptr(cols["b"]),
-                                         _abi.ptr(cols["read_id"]), _abi.ptr(cols["c"]), _abi.ptr(po), _abi.ptr(pc)))
-        sigs[name] = {c: v[:k] for c, v in cols.items()}
-        if name == "INS":
-            poff, pcnt = po[:k], pc[:k]
-    npz = C.c_int64(0)
-    _lib.check(self.L.csv_fetch_pieces(self.h, C.c_int64(0), None, C.byref(npz)))
-    pieces = np.zeros((max(npz.value, 1), 4), dtype=np.int32)
-    _lib.check(self.L.csv_fetch_pieces(self.h, C.c_int64(len(pieces)), _abi.ptr(pieces), C.byref(npz)))
-    nr = self._ex_rows
-    rows = {k: np.zeros(max(nr, 1), dtype=np.int32) for k in ("chrom", "start", "end", "read_id")}
-    prim = np.zeros(max(nr, 1), dtype=np.uint8)
-    _lib.check(self.L.csv_fetch_read_rows(self.h, C.c_int64(max(nr, 1)), _abi.ptr(rows["chrom"]), _abi.ptr(rows["start"]), _abi.ptr(rows["end"]),
-                                          _abi.ptr(rows["read_id"]), prim.ctypes.data_as(C.POINTER(C.c_uint8))))
-    rows = {k: v[:nr] for k, v in rows.items()}
-    rows["is_primary"] = prim[:nr]
-    return dict(sigs=sigs, piece_off=poff, piece_cnt=pcnt, pieces=pieces[:npz.value], rows=rows)
-
-
-Engine.pin_packet = _pin_packet_method
-Engine.extract_reset = _extract_reset_method
-Engine.extract_skipped = _extract_skipped_method
-Engine.fetch_ins_pieces = _fetch_ins_pieces_method
-Engine.fetch_sig_cols = _fetch_sig_cols_method
-Engine.remap_read_ids = _remap_read_ids_method
-Engine.fetch_read_rows = _fetch_read_rows_method
-Engine.swap_ins_rows = _swap_ins_rows_method
-Engine.extract = _extract_method
-Engine.fetch_ins_seqs = _fetch_ins_seqs_method
-Engine.ins_seq_tensors = _ins_seq_tensors_method
-Engine.fetch_extracted = _fetch_extracted_method
-Engine.rank_names = _rank_names_method
-Engine.fetch_names = _fetch_names_method
-Engine.name_rank_tensor = _name_rank_tensor_method
-Engine.order_ins_ties = _order_ins_ties_method
-Engine.set_scan_regions = _set_scan_regions_method
-Engine.fetch_alignments = _fetch_alignments_method
-Engine.scan = _scan_method
