@@ -1245,9 +1245,14 @@ __global__ void __launch_bounds__(256) k_reads_pass(GenoJob G, PairBuf PB, const
     constexpr int TAB = 1024;            // contigs whose (offset, validity) live in shared memory
     __shared__ uint32_t s_warp[10];
     __shared__ uint64_t s_off[TAB];      // linear offset, ~0 for a contig outside the shard
+    __shared__ uint32_t s_lim[TAB];      // len + pad - 1: where a row's end is cut (the contig's linear range ends there)
     __shared__ uint8_t s_seen[TAB];
     const int n_tab = G.ct.n < TAB ? G.ct.n : TAB;
-    for (int i = threadIdx.x; i < n_tab; i += 256) { s_off[i] = G.ct.len[i] < 0 ? ~0ull : G.ct.off[i]; s_seen[i] = 0; }
+    for (int i = threadIdx.x; i < n_tab; i += 256) {
+        s_off[i] = G.ct.len[i] < 0 ? ~0ull : G.ct.off[i];
+        s_lim[i] = (uint32_t)(G.ct.off[i + 1] - G.ct.off[i] - 1);
+        s_seen[i] = 0;
+    }
     __syncthreads();
     const int64_t n_tiles = (n_reads + 256 * ITEMS - 1) / (256 * ITEMS);
     for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -1286,18 +1291,26 @@ __global__ void __launch_bounds__(256) k_reads_pass(GenoJob G, PairBuf PB, const
             if (r >= n_reads) continue;
             if (ch[j] < 0 || ch[j] >= G.ct.n) { atomicOr(status, ST_BAD_CHROM); continue; }
             uint64_t off;
+            uint32_t lim;
             if (ch[j] < TAB) {
                 off = s_off[ch[j]];
+                lim = s_lim[ch[j]];
                 // deliberate benign race (racecheck reports it): a byte that only goes 0 -> 1, every writer stores the same value, read
                 // after the final __syncthreads().  The race-free variants (shared atomics) cost 10 registers = one CTA per SM in this
                 // latency-bound pass.
                 if (!s_seen[ch[j]]) s_seen[ch[j]] = 1;
             } else {
                 off = G.ct.len[ch[j]] < 0 ? ~0ull : G.ct.off[ch[j]];
+                lim = (uint32_t)(G.ct.off[ch[j] + 1] - G.ct.off[ch[j]] - 1);
                 if (!G.has_rows[ch[j]]) G.has_rows[ch[j]] = 1;
             }
             if (off == ~0ull) { atomicOr(status, ST_BAD_CHROM); continue; }   // outside the shard
+            if (st[j] < 0 || en[j] < st[j]) { atomicOr(status, ST_BAD_POS); continue; }
             if (!pr[j]) continue;
+            // A row that ends past its contig would reach the first windows of the next contig in the linear coordinate: it ends
+            // at the last linear coordinate of its own contig instead (DESIGN §3: exact for INS / DEL windows, which end there at
+            // the latest).  Both paths of the pair test (pair buffer and inline) use this end.
+            if ((uint32_t)en[j] > lim) en[j] = (int32_t)lim;
             const uint64_t RS = off + (uint64_t)(uint32_t)st[j], RE = off + (uint64_t)(uint32_t)en[j];
             lin[j] = RS;
             const uint32_t b0 = (uint32_t)(RS >> G.shift);
@@ -1320,7 +1333,7 @@ __global__ void __launch_bounds__(256) k_reads_pass(GenoJob G, PairBuf PB, const
             if (!cnt[j]) continue;
             const int64_t r = RP_ROW(j);
             const int32_t rid = r_id[r];
-            const uint64_t RS = lin[j], RE = lin[j] + (uint64_t)(uint32_t)(en[j] - st[j]);
+            const uint64_t RS = lin[j], RE = lin[j] - (uint64_t)(uint32_t)st[j] + (uint64_t)(uint32_t)en[j];
             // slots below the capacity go to the pair buffer (every reserved slot < cap MUST be written:
             // k_pairs_test consumes [0, min(count, cap))); the rest is tested inline (correct, just slower)
             uint32_t k = 0;
@@ -1353,8 +1366,11 @@ __global__ void __launch_bounds__(256) k_pairs_test(GenoJob G, PairBuf PB, const
             test_pair32(G, pr.x, pr.y, (int32_t)pr.z, pr.w);
         } else {
             const uint2 pr = PB.pairs[p];
-            const uint64_t off = G.ct.off[r_chrom[pr.x]];
-            test_pair(G, off + (uint64_t)(uint32_t)r_start[pr.x], off + (uint64_t)(uint32_t)r_end[pr.x], r_id[pr.x], pr.y);
+            const int32_t ch = r_chrom[pr.x];
+            const uint64_t off = G.ct.off[ch];
+            // the row's end clamped to its contig as in k_reads_pass (the pair carries only the row index)
+            const uint64_t RE = min(off + (uint64_t)(uint32_t)r_end[pr.x], G.ct.off[ch + 1] - 1);
+            test_pair(G, off + (uint64_t)(uint32_t)r_start[pr.x], RE, r_id[pr.x], pr.y);
         }
     }
 }

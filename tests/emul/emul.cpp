@@ -199,9 +199,12 @@ extern "C" int emul_cluster(const csv_params* P, int32_t n_contigs, const int64_
         std::vector<uint32_t> fill(nb, 0);
         for (auto& x : wl) wsorted[bstart[x.first] + fill[x.first]++] = x.second;
         for (int64_t r = 0; reads && r < reads->n; r++) {
+            if (reads->start[r] < 0 || reads->end[r] < reads->start[r]) { fprintf(stderr, "emul: reads row %lld: end < start\n", (long long)r); return CSV_E_INPUT; }
             has_rows[reads->chrom[r]] = 1;
             if (!reads->is_primary[r]) continue;
-            const uint64_t RS = cx.off[reads->chrom[r]] + (uint64_t)reads->start[r], RE = cx.off[reads->chrom[r]] + (uint64_t)reads->end[r];
+            // the row's end clamped to the last linear coordinate of its contig (k_reads_pass)
+            const uint64_t RS = cx.off[reads->chrom[r]] + (uint64_t)reads->start[r];
+            const uint64_t RE = std::min(cx.off[reads->chrom[r]] + (uint64_t)reads->end[r], cx.off[reads->chrom[r] + 1] - 1);
             for (uint64_t b = RS >> shift; b <= (RE >> shift) && b < nb; b++)
                 for (uint32_t w = bstart[b]; w < bstart[b + 1]; w++) {
                     const csv_cand& c = cands[wsorted[w].cand];

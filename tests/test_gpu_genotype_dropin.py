@@ -9,6 +9,7 @@ import pytest
 
 import genotype_golden as gg
 import golden_util
+from genotype_edges import windows_of_candidates
 from cutesv_b200 import _abi, runtime
 from cutesv_b200._lib import CuteSVError
 from oracle import compare_records
@@ -117,21 +118,6 @@ def test_random_multi_contig_matches_numpy(engine):
     ref = engine.cal_gl(dr, [len(x) for x in sup])
     for k in ("gt", "pl", "gq", "qual"):
         assert np.array_equal(g[k], ref[k]), k
-
-
-def windows_of_candidates(cands, p):
-    """csv_cluster's genotype windows (call_gt of resolveINDEL.py:450-451, resolveDUP.py:146-151, resolveINV.py:218-221), half units."""
-    t = cands["svtype"]
-    w = np.zeros((len(cands), 2), dtype=_abi.WINDOW_DTYPE)
-    w["chrom"] = cands["chrom"][:, None]
-    b = np.where(t == _abi.CSV_INS, p.gt_bias_ins, p.bias_del).astype(np.int64)
-    sp = cands["search_pos"].astype(np.int64)
-    w["s2"][:, 0], w["e2"][:, 0] = 2 * np.maximum(sp - b, 0), 2 * (sp + b)
-    nb = np.where(t == _abi.CSV_DUP, np.minimum(p.bias_dup, cands["pos2"].astype(np.int64) - cands["pos"]), p.bias_inv)
-    for k, x in ((0, cands["pos"].astype(np.int64)), (1, cands["pos2"].astype(np.int64))):
-        two = (t == _abi.CSV_DUP) | (t == _abi.CSV_INV)
-        w["s2"][two, k], w["e2"][two, k] = np.maximum(2 * x - nb, 0)[two], (2 * x + nb)[two]
-    return w
 
 
 @pytest.mark.parametrize("name", ["cfg2_s0p002", "cfg3_s0p004"])
