@@ -248,6 +248,7 @@ struct csv_ctx {
     bool profiling = false;
     // csv_set_profiling(c, 2): no per-launch events (programmatic launches, the side streams and the lanes run as they do
     // unprofiled; no graph replay), only one interval per INS / DEL lane from the end of the density filter to the lane's end
+    // and one ("tail") from the lane join to the end of the chain
     bool lane_marks = false;
     struct Interval { int st; cudaEvent_t a, b; int64_t bytes; };
     std::vector<Interval> ivs;
@@ -1415,6 +1416,8 @@ static int enqueue_cluster(csv_ctx* c, uint32_t type_mask) {
     rc = join_lanes(c);
     if (rc) return rc;
     if (aux_used) CU(cudaStreamWaitEvent(c->stream, c->ev_aux, 0));
+    int tail_mark = -1;   // lane_marks: the serial tail, from the lane join to the end of the call's chain
+    if (c->lane_marks) { kprof_begin(c, c->stream, "tail"); tail_mark = (int)c->kivs.size() - 1; }
     GenoJob G;
     memset(&G, 0, sizeof(G));
     G.cand = c->cand.as<csv_cand>(); G.geno = c->geno.as<csv_geno>(); G.names = c->names.as<int32_t>(); G.ctr = ctr;
@@ -1503,6 +1506,7 @@ static int enqueue_cluster(csv_ctx* c, uint32_t type_mask) {
         }
     }
     stage_end(c, c->stream, CSV_ST_GENOTYPE);
+    if (tail_mark >= 0) CU(cudaEventRecord(c->kivs[tail_mark].b, c->stream));
     return CSV_OK;
 }
 

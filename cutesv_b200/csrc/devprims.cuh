@@ -112,14 +112,29 @@ __device__ __forceinline__ uint32_t block_excl_scan_256(uint32_t v, uint32_t* s_
 // Unordered append: every thread of a 256-thread CTA asks for `cnt` slots of a global buffer; ONE
 // atomicAdd per CTA reserves the whole range (same-address returning atomics serialise at the L2
 // slice, so one per warp would cost more than the scan).  Returns the thread's first slot.
-__device__ __forceinline__ uint32_t block_reserve_256(uint32_t cnt, uint32_t* counter, uint32_t* s_warp /*10 words*/) {
-    uint32_t total;
-    const uint32_t local = block_excl_scan_256(cnt, s_warp, &total);
-    if (threadIdx.x == 0) s_warp[9] = total ? atomicAdd(counter, total) : 0u;
+// Two barriers per call: the warp totals go to the half of s_warp that `parity` selects, and a caller that calls it in a
+// loop flips `parity` every call, so the next call's writes never meet this call's reads and no third barrier is needed.
+__device__ __forceinline__ uint32_t block_reserve_256(uint32_t cnt, uint32_t* counter, uint32_t* s_warp /*17 words*/, int parity) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    uint32_t incl = cnt;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const uint32_t y = __shfl_up_sync(0xffffffffu, incl, d);
+        if (lane >= d) incl += y;
+    }
+    uint32_t* part = s_warp + 8 * parity;
+    if (lane == 31) part[warp] = incl;
     __syncthreads();
-    const uint32_t base = s_warp[9];
+    uint32_t before = 0, total = 0;
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+        const uint32_t t = part[i];
+        before += i < warp ? t : 0u;
+        total += t;
+    }
+    if (threadIdx.x == 0) s_warp[16] = total ? atomicAdd(counter, total) : 0u;
     __syncthreads();
-    return base + local;
+    return s_warp[16] + before + incl - cnt;
 }
 
 static constexpr int SEL_THREADS = 256;

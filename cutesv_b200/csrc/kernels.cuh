@@ -1184,6 +1184,24 @@ __global__ void k_windows(GenoJob G) {
     }
 }
 
+// Is `rid` one of names[off, off + n)?  The slice is read as the 16 B-aligned quads that hold it, two per step (a names
+// slice is about 22 ids on config 2: at most four steps instead of 22 scattered 4 B loads); ids of a quad outside the slice are
+// masked out by index.  The quads stay inside the buffer: DBuf allocations end at least 256 B past the bytes asked for.
+__device__ __forceinline__ bool names_contain(const int32_t* __restrict__ names, int32_t off, int32_t n, int32_t rid) {
+    const int lead = off & 3;
+    const int4* q = reinterpret_cast<const int4*>(names + (off - lead));
+    const int end = lead + n;   // the slice is ints [lead, end) of the quads from q on
+    bool found = false;
+    for (int b = 0; b < end && !found; b += 8) {
+        const int4 x = __ldg(q + (b >> 2));
+        const int4 y = b + 4 < end ? __ldg(q + (b >> 2) + 1) : make_int4(0, 0, 0, 0);
+        const int32_t v[8] = {x.x, x.y, x.z, x.w, y.x, y.y, y.z, y.w};
+#pragma unroll
+        for (int k = 0; k < 8; k++) found |= v[k] == rid && b + k >= lead && b + k < end;
+    }
+    return found;
+}
+
 // One (read, window) test of assign_gt / overlap_cover: a primary read covers window [s,e] iff
 // start <= s and end >= e (cuteSV_genotype.py:100-138); DR counts covering reads that are not
 // supporting reads (:161-173).  RS/RE are linear coordinates.
@@ -1199,15 +1217,7 @@ __device__ __forceinline__ void test_pair(const GenoJob& G, uint64_t RS, uint64_
         window_of(c, 0, G.gp, &s0, &e0);
         if (RS <= coff + (uint64_t)s0 && RE >= coff + (uint64_t)e0) return;
     }
-    // supporting reads are not counted; four independent loads per step instead of a load-compare-branch chain
-    const int32_t* nm = G.names + c.names_off;
-    const int n = c.names_cnt;
-    bool found = false;
-    int k = 0;
-    for (; k + 4 <= n && !found; k += 4)
-        found = (__ldg(nm + k) == rid) | (__ldg(nm + k + 1) == rid) | (__ldg(nm + k + 2) == rid) | (__ldg(nm + k + 3) == rid);
-    for (; k < n && !found; k++) found = __ldg(nm + k) == rid;
-    if (!found) atomicAdd(&G.dr[ent >> 1], 1u);
+    if (!names_contain(G.names, c.names_off, c.names_cnt, rid)) atomicAdd(&G.dr[ent >> 1], 1u);   // supporting reads are not counted
 }
 
 // the same test on a WinRec (32-bit linear coordinates): one 32 B gather instead of the candidate record, its contig
@@ -1216,14 +1226,7 @@ __device__ __forceinline__ void test_pair32(const GenoJob& G, uint32_t RS, uint3
     const uint4 lo = __ldg(reinterpret_cast<const uint4*>(&G.win_rec[w])), hi = __ldg(reinterpret_cast<const uint4*>(&G.win_rec[w]) + 1);
     if (!(RS <= lo.x && RE >= lo.y)) return;
     if (hi.w && RS <= lo.z && RE >= lo.w) return;   // union of the two breakpoint covers (resolveDUP.py:155-157): count once
-    const int32_t* nm = G.names + (int32_t)hi.x;
-    const int n = (int32_t)hi.y;
-    bool found = false;
-    int k = 0;
-    for (; k + 4 <= n && !found; k += 4)
-        found = (__ldg(nm + k) == rid) | (__ldg(nm + k + 1) == rid) | (__ldg(nm + k + 2) == rid) | (__ldg(nm + k + 3) == rid);
-    for (; k < n && !found; k++) found = __ldg(nm + k) == rid;
-    if (!found) atomicAdd(&G.dr[hi.z], 1u);
+    if (!names_contain(G.names, (int32_t)hi.x, (int32_t)hi.y, rid)) atomicAdd(&G.dr[hi.z], 1u);
 }
 
 // ONE streaming pass over the reads table (replaces overlap_cover's event sort + sweep,
@@ -1240,114 +1243,156 @@ __global__ void __launch_bounds__(256) k_reads_pass(GenoJob G, PairBuf PB, const
                                                     const int32_t* __restrict__ r_start, const int32_t* __restrict__ r_end,
                                                     const int32_t* __restrict__ r_id, const uint8_t* __restrict__ r_prim,
                                                     int64_t n_reads, uint32_t* status) {
+    // LIN32: linear coordinates and contig offsets in 32 bits (every offset < 2^32 - 4096, so ~0 stays a free marker)
+    using Lin = typename std::conditional<LIN32, uint32_t, uint64_t>::type;
     pdl_launch_dependents(); pdl_wait();   // programmatic dependent launch: resident early, starts when the previous kernel has finished
-    constexpr int ITEMS = 4;
+    constexpr int ITEMS = 4;             // four consecutive rows per thread: one 128-bit load per column
     constexpr int TAB = 1024;            // contigs whose (offset, validity) live in shared memory
-    __shared__ uint32_t s_warp[10];
-    __shared__ uint64_t s_off[TAB];      // linear offset, ~0 for a contig outside the shard
+    constexpr Lin NO_OFF = ~(Lin)0;
+    __shared__ uint32_t s_warp[17];
+    __shared__ Lin s_off[TAB];           // linear offset, NO_OFF for a contig outside the shard
     __shared__ uint32_t s_lim[TAB];      // len + pad - 1: where a row's end is cut (the contig's linear range ends there)
     __shared__ uint8_t s_seen[TAB];
     const int n_tab = G.ct.n < TAB ? G.ct.n : TAB;
     for (int i = threadIdx.x; i < n_tab; i += 256) {
-        s_off[i] = G.ct.len[i] < 0 ? ~0ull : G.ct.off[i];
+        s_off[i] = G.ct.len[i] < 0 ? NO_OFF : (Lin)G.ct.off[i];
         s_lim[i] = (uint32_t)(G.ct.off[i + 1] - G.ct.off[i] - 1);
         s_seen[i] = 0;
     }
     __syncthreads();
+    const bool aligned = ((((uintptr_t)r_chrom) | ((uintptr_t)r_start) | ((uintptr_t)r_end) | ((uintptr_t)r_id)) & 15) == 0 &&
+                         (((uintptr_t)r_prim) & 3) == 0;
     const int64_t n_tiles = (n_reads + 256 * ITEMS - 1) / (256 * ITEMS);
-    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        const int64_t base = tile * 256 * ITEMS;
-        int32_t ch[ITEMS], st[ITEMS], en[ITEMS];
-        uint8_t pr[ITEMS];
-        // row of item j: four consecutive rows per thread (one 128-bit load per column) when the columns allow it
-        const int64_t r0 = base + (int64_t)threadIdx.x * ITEMS;
-        const bool vec = ITEMS == 4 && r0 + ITEMS <= n_reads &&
-                         ((((uintptr_t)r_chrom) | ((uintptr_t)r_start) | ((uintptr_t)r_end)) & 15) == 0 && (((uintptr_t)r_prim) & 3) == 0;
-        const bool blocked = __syncthreads_and(vec || r0 >= n_reads) != 0;   // one mapping per tile (uniform: the pair slots are reserved per CTA)
-#define RP_ROW(j) (blocked ? r0 + (j) : base + (int64_t)(j) * 256 + threadIdx.x)
-        if (blocked && vec) {
+    // the columns of the thread's rows in the next tile: loaded one tile ahead, so that a tile's HBM latency overlaps the
+    // probe, the reservation and the pair stores of the tile before it
+    int32_t ch[ITEMS], st[ITEMS], en[ITEMS], id[ITEMS];
+    uint32_t pr = 0;
+    auto load = [&](int64_t tile) {
+        const int64_t r0 = tile * 256 * ITEMS + (int64_t)threadIdx.x * ITEMS;
+        if (aligned && r0 + ITEMS <= n_reads) {
             const int4 c4 = __ldcs(reinterpret_cast<const int4*>(r_chrom + r0)), s4 = __ldcs(reinterpret_cast<const int4*>(r_start + r0));
-            const int4 e4 = __ldcs(reinterpret_cast<const int4*>(r_end + r0));
-            const uint32_t p4 = __ldcs(reinterpret_cast<const uint32_t*>(r_prim + r0));
+            const int4 e4 = __ldcs(reinterpret_cast<const int4*>(r_end + r0)), i4 = __ldcs(reinterpret_cast<const int4*>(r_id + r0));
+            pr = __ldcs(reinterpret_cast<const uint32_t*>(r_prim + r0));
             ch[0] = c4.x; ch[1] = c4.y; ch[2] = c4.z; ch[3] = c4.w;
             st[0] = s4.x; st[1] = s4.y; st[2] = s4.z; st[3] = s4.w;
             en[0] = e4.x; en[1] = e4.y; en[2] = e4.z; en[3] = e4.w;
-            pr[0] = (uint8_t)p4; pr[1] = (uint8_t)(p4 >> 8); pr[2] = (uint8_t)(p4 >> 16); pr[3] = (uint8_t)(p4 >> 24);
+            id[0] = i4.x; id[1] = i4.y; id[2] = i4.z; id[3] = i4.w;
+        } else {
+            pr = 0;
+#pragma unroll
+            for (int j = 0; j < ITEMS; j++) {
+                const int64_t r = r0 + j;
+                const bool in = r < n_reads;
+                ch[j] = in ? __ldcs(r_chrom + r) : -1; st[j] = in ? __ldcs(r_start + r) : 0; en[j] = in ? __ldcs(r_end + r) : 0;
+                id[j] = in ? __ldcs(r_id + r) : 0;
+                pr |= (uint32_t)(in ? __ldcs(r_prim + r) : 0) << (8 * j);
+            }
+        }
+    };
+    if ((int64_t)blockIdx.x < n_tiles) load(blockIdx.x);
+    int parity = 0;
+    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, parity ^= 1) {
+        const int64_t r0 = tile * 256 * ITEMS + (int64_t)threadIdx.x * ITEMS;
+        int32_t cid[ITEMS];
+        uint32_t b0[ITEMS], b1[ITEMS];
+        Lin RS[ITEMS], RE[ITEMS];
+        // a primary row's linear range and bin range; a row that ends past its contig would reach the first windows of the
+        // next contig in the linear coordinate: it ends at the last linear coordinate of its own contig instead (DESIGN §3:
+        // exact for INS / DEL windows, which end there at the latest).  Both paths of the pair test (pair buffer and inline)
+        // use this end.  Other rows get an empty bin range: no probe, no pairs.
+        auto place = [&](int j, Lin off, uint32_t lim, bool prim) {
+            RS[j] = off + (Lin)(uint32_t)st[j];
+            RE[j] = off + (Lin)((uint32_t)en[j] > lim ? lim : (uint32_t)en[j]);
+            b0[j] = prim ? (uint32_t)(RS[j] >> G.shift) : 1u;
+            b1[j] = prim ? min((uint32_t)(RE[j] >> G.shift), G.n_bins - 1) : 0u;
+        };
+        // common case, one vote per warp: every row of the warp exists and is valid and its contig is in the shared table
+        bool ok = r0 + ITEMS <= n_reads;
+#pragma unroll
+        for (int j = 0; j < ITEMS; j++)
+            ok = ok && (uint32_t)ch[j] < (uint32_t)n_tab && s_off[ch[j]] != NO_OFF && st[j] >= 0 && en[j] >= st[j];
+        if (__all_sync(0xffffffffu, ok)) {
+#pragma unroll
+            for (int j = 0; j < ITEMS; j++) {
+                const int32_t c = ch[j];
+                cid[j] = id[j];
+                // deliberate benign race (racecheck reports it): a byte that only goes 0 -> 1, every writer stores the same
+                // value, read after the final __syncthreads().  The race-free variants (shared atomics) cost registers, and
+                // so resident CTAs, in this latency-bound pass.
+                s_seen[c] = 1;
+                place(j, s_off[c], s_lim[c], ((pr >> (8 * j)) & 0xffu) != 0);
+            }
         } else {
 #pragma unroll
             for (int j = 0; j < ITEMS; j++) {
-                const int64_t r = RP_ROW(j);
-                const bool in = r < n_reads;
-                ch[j] = in ? __ldcs(r_chrom + r) : -1; st[j] = in ? __ldcs(r_start + r) : 0; en[j] = in ? __ldcs(r_end + r) : 0;
-                pr[j] = in ? __ldcs(r_prim + r) : 0;
+                const int32_t c = ch[j], s = st[j], e = en[j];
+                cid[j] = id[j];
+                b0[j] = 1; b1[j] = 0; RS[j] = 0; RE[j] = 0;
+                if (r0 + j >= n_reads) continue;
+                if (c < 0 || c >= G.ct.n) { atomicOr(status, ST_BAD_CHROM); continue; }
+                Lin off;
+                uint32_t lim;
+                if (c < TAB) {
+                    off = s_off[c];
+                    lim = s_lim[c];
+                    if (!s_seen[c]) s_seen[c] = 1;
+                } else {
+                    off = G.ct.len[c] < 0 ? NO_OFF : (Lin)G.ct.off[c];
+                    lim = (uint32_t)(G.ct.off[c + 1] - G.ct.off[c] - 1);
+                    if (!G.has_rows[c]) G.has_rows[c] = 1;
+                }
+                if (off == NO_OFF) { atomicOr(status, ST_BAD_CHROM); continue; }   // outside the shard
+                if (s < 0 || e < s) { atomicOr(status, ST_BAD_POS); continue; }
+                place(j, off, lim, ((pr >> (8 * j)) & 0xffu) != 0);
             }
         }
-        uint32_t w[ITEMS], cnt[ITEMS], total = 0;
-        uint64_t lin[ITEMS];   // RS of the read
+        if ((int64_t)tile + gridDim.x < n_tiles) load(tile + gridDim.x);
+        // any occupied bin in [b0, b1]?  The first and last words of the bit map for every row are loaded before any is
+        // tested; a read spans at most two words unless it covers more than 32 bins.
+        uint32_t m[ITEMS], m1[ITEMS];
 #pragma unroll
         for (int j = 0; j < ITEMS; j++) {
-            w[j] = 0; cnt[j] = 0; lin[j] = 0;
-            const int64_t r = RP_ROW(j);
-            if (r >= n_reads) continue;
-            if (ch[j] < 0 || ch[j] >= G.ct.n) { atomicOr(status, ST_BAD_CHROM); continue; }
-            uint64_t off;
-            uint32_t lim;
-            if (ch[j] < TAB) {
-                off = s_off[ch[j]];
-                lim = s_lim[ch[j]];
-                // deliberate benign race (racecheck reports it): a byte that only goes 0 -> 1, every writer stores the same value, read
-                // after the final __syncthreads().  The race-free variants (shared atomics) cost 10 registers = one CTA per SM in this
-                // latency-bound pass.
-                if (!s_seen[ch[j]]) s_seen[ch[j]] = 1;
-            } else {
-                off = G.ct.len[ch[j]] < 0 ? ~0ull : G.ct.off[ch[j]];
-                lim = (uint32_t)(G.ct.off[ch[j] + 1] - G.ct.off[ch[j]] - 1);
-                if (!G.has_rows[ch[j]]) G.has_rows[ch[j]] = 1;
+            m[j] = m1[j] = 0;
+            if (b0[j] <= b1[j]) {
+                m[j] = __ldg(&G.bin_bits[b0[j] >> 5]);
+                if ((b1[j] >> 5) != (b0[j] >> 5)) m1[j] = __ldg(&G.bin_bits[b1[j] >> 5]);
             }
-            if (off == ~0ull) { atomicOr(status, ST_BAD_CHROM); continue; }   // outside the shard
-            if (st[j] < 0 || en[j] < st[j]) { atomicOr(status, ST_BAD_POS); continue; }
-            if (!pr[j]) continue;
-            // A row that ends past its contig would reach the first windows of the next contig in the linear coordinate: it ends
-            // at the last linear coordinate of its own contig instead (DESIGN §3: exact for INS / DEL windows, which end there at
-            // the latest).  Both paths of the pair test (pair buffer and inline) use this end.
-            if ((uint32_t)en[j] > lim) en[j] = (int32_t)lim;
-            const uint64_t RS = off + (uint64_t)(uint32_t)st[j], RE = off + (uint64_t)(uint32_t)en[j];
-            lin[j] = RS;
-            const uint32_t b0 = (uint32_t)(RS >> G.shift);
-            uint32_t b1 = (uint32_t)(RE >> G.shift);
-            if (b1 >= G.n_bins) b1 = G.n_bins - 1;
-            if (b0 > b1) continue;
-            // any occupied bin in [b0, b1]?  One or two words of the bit map for a typical read.
-            const uint32_t w0 = b0 >> 5, w1 = b1 >> 5;
-            uint32_t m = __ldg(&G.bin_bits[w0]) & (0xffffffffu << (b0 & 31));
-            if (w1 == w0) m &= 0xffffffffu >> (31 - (b1 & 31));
+        }
+        uint32_t lo[ITEMS], hi[ITEMS];
+#pragma unroll
+        for (int j = 0; j < ITEMS; j++) {
+            lo[j] = hi[j] = 0;
+            if (b0[j] > b1[j]) continue;
+            const uint32_t w0 = b0[j] >> 5, w1 = b1[j] >> 5;
+            uint32_t x = m[j] & (0xffffffffu << (b0[j] & 31));
+            if (w1 == w0) x &= 0xffffffffu >> (31 - (b1[j] & 31));
             else {
-                for (uint32_t wi = w0 + 1; wi < w1 && !m; wi++) m = __ldg(&G.bin_bits[wi]);
-                if (!m) m = __ldg(&G.bin_bits[w1]) & (0xffffffffu >> (31 - (b1 & 31)));
+                x |= m1[j] & (0xffffffffu >> (31 - (b1[j] & 31)));
+                for (uint32_t wi = w0 + 1; wi < w1 && !x; wi++) x = __ldg(&G.bin_bits[wi]);
             }
-            if (m) { w[j] = G.bin_start[b0]; cnt[j] = G.bin_start[b1 + 1] - w[j]; total += cnt[j]; }
+            if (x) { lo[j] = G.bin_start[b0[j]]; hi[j] = G.bin_start[b1[j] + 1]; }
         }
-        uint32_t o = block_reserve_256(total, PB.count, s_warp);
+        uint32_t total = 0;
+#pragma unroll
+        for (int j = 0; j < ITEMS; j++) total += hi[j] - lo[j];
+        uint32_t o = block_reserve_256(total, PB.count, s_warp, parity);
 #pragma unroll
         for (int j = 0; j < ITEMS; j++) {
-            if (!cnt[j]) continue;
-            const int64_t r = RP_ROW(j);
-            const int32_t rid = r_id[r];
-            const uint64_t RS = lin[j], RE = lin[j] - (uint64_t)(uint32_t)st[j] + (uint64_t)(uint32_t)en[j];
+            const uint32_t cnt = hi[j] - lo[j];
+            if (!cnt) continue;
             // slots below the capacity go to the pair buffer (every reserved slot < cap MUST be written:
             // k_pairs_test consumes [0, min(count, cap))); the rest is tested inline (correct, just slower)
             uint32_t k = 0;
-            for (; k < cnt[j] && (uint64_t)o + k < PB.cap; k++) {
-                if (LIN32) PB.pairs4[o + k] = make_uint4((uint32_t)RS, (uint32_t)RE, (uint32_t)rid, w[j] + k);
-                else PB.pairs[o + k] = make_uint2((uint32_t)r, w[j] + k);
+            for (; k < cnt && (uint64_t)o + k < PB.cap; k++) {
+                if (LIN32) PB.pairs4[o + k] = make_uint4((uint32_t)RS[j], (uint32_t)RE[j], (uint32_t)cid[j], lo[j] + k);
+                else PB.pairs[o + k] = make_uint2((uint32_t)(r0 + j), lo[j] + k);
             }
-            for (; k < cnt[j]; k++) {
-                if (LIN32) test_pair32(G, (uint32_t)RS, (uint32_t)RE, rid, w[j] + k);
-                else test_pair(G, RS, RE, rid, w[j] + k);
+            for (; k < cnt; k++) {
+                if (LIN32) test_pair32(G, (uint32_t)RS[j], (uint32_t)RE[j], cid[j], lo[j] + k);
+                else test_pair(G, RS[j], RE[j], cid[j], lo[j] + k);
             }
-            o += cnt[j];
+            o += cnt;
         }
-#undef RP_ROW
     }
     __syncthreads();
     for (int i = threadIdx.x; i < n_tab; i += 256)

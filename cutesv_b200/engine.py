@@ -45,7 +45,8 @@ class Engine(object):
         _lib.check(self.L.csv_set_contigs(self.h, C.c_int32(len(lens)), lens.ctypes.data_as(C.POINTER(C.c_int64))))
 
     def set_profiling(self, on):
-        """True: every launch between CUDA events.  "lanes": only the INS / DEL back-end intervals, launches as unprofiled."""
+        """True: every launch between CUDA events.  "lanes": only the INS / DEL back-end intervals and the
+        serial tail after the lane join ("tail"), launches as unprofiled."""
         _lib.check(self.L.csv_set_profiling(self.h, 2 if on == "lanes" else int(bool(on))))
 
     def set_lanes(self, on):
