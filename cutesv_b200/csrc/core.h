@@ -1303,4 +1303,63 @@ CSV_HD void pf_strip_offsets(const H& h, int b0, int n, uint64_t flags, uint32_t
     }
 }
 
+// ------------------------------------------------------------------------------------------
+// INS/DEL chain clusters of one k_select_heads tile, read from its link mask: bit q (word q >> 5, bit q & 31) is set
+// when element q is chained to element q - 1.  The caller's mask holds a halo of words on both sides of the tile and
+// indexes it so that every q these routines read stays inside it.
+// ------------------------------------------------------------------------------------------
+#if defined(__CUDA_ARCH__)
+CSV_D int ctz32(uint32_t x) { return __ffs((int)x) - 1; }
+CSV_D int clz32(uint32_t x) { return __clz((int)x); }
+#else
+inline int ctz32(uint32_t x) { return __builtin_ctz(x); }
+inline int clz32(uint32_t x) { return __builtin_clz(x); }
+#endif
+
+// set bits q, q + 1, ... up to the first clear one, at most cap (reads bits q .. q + cap + 31 at most)
+CSV_HD int link_run_up(const uint32_t* link, int q, int cap) {
+    int r = 0;
+    while (r < cap) {
+        const int bo = q & 31;
+        const uint32_t z = ~(link[q >> 5] >> bo);   // bit k: bit q + k is clear; the 32 - bo vacated bits count as clear
+        const int ones = z ? ctz32(z) : 32;
+        r += ones;
+        if (ones < 32 - bo) break;
+        q += 32 - bo;
+    }
+    return r < cap ? r : cap;
+}
+
+// set bits q, q - 1, ... down to the first clear one, at most cap (reads bits q - cap - 31 .. q at most)
+CSV_HD int link_run_down(const uint32_t* link, int q, int cap) {
+    int r = 0;
+    while (r < cap) {
+        const int bo = q & 31;
+        const uint32_t z = ~(link[q >> 5] << (31 - bo));   // bit 31 - k: bit q - k is clear; the vacated bits count as clear
+        const int ones = z ? clz32(z) : 32;
+        r += ones;
+        if (ones < bo + 1) break;
+        q -= bo + 1;
+    }
+    return r < cap ? r : cap;
+}
+
+// q starts a chain cluster of at least need members: it is not chained to q - 1, and q + 1 .. q + need - 1 are chained
+CSV_HD bool chain_head(const uint32_t* link, int q, int need) {
+    return !((link[q >> 5] >> (q & 31)) & 1u) && link_run_up(link, q + 1, need - 1) >= need - 1;
+}
+
+// q is a member of a chain cluster of at least need members, wherever its head lies: the chained steps before and after
+// q, each counted up to need - 1, make need - 1 together
+CSV_HD bool chain_member(const uint32_t* link, int q, int need) {
+    return link_run_down(link, q, need - 1) + link_run_up(link, q + 1, need - 1) >= need - 1;
+}
+
+// size class of the cluster headed at q: its member count when it has at most 32 members, 33 for up to split members,
+// 34 beyond (reads the forward run up to split links)
+CSV_HD int chain_size_class(const uint32_t* link, int q, int split) {
+    const int m = 1 + link_run_up(link, q + 1, split);
+    return m <= 32 ? m : m <= split ? 33 : 34;
+}
+
 }  // namespace csv

@@ -1012,6 +1012,7 @@ static int run_segment_and_cluster(csv_ctx* c, Lane& L, TypeJob& J, int t, uint3
         if ((t == CSV_DEL || t == CSV_INS) && J.iv.rec) {
             MR.rec = const_cast<IndelRec*>(J.iv.rec); MR.recc = const_cast<int32_t*>(J.iv.recc);
             MR.a = J.iv.a; MR.b = J.iv.b; MR.rid = J.iv.rid; MR.c = J.iv.recc ? J.iv.c : nullptr; MR.sidx = J.iv.sidx;
+            if (t == CSV_DEL && J.keys32) { MR.del_off = c->d_off.as<uint64_t>(); MR.n_contigs = c->n_contigs; }
             if (J.cp.keep >= 1.0 && J.small_path) {   // the walk also sorts the kept clusters into the two lists of the cluster kernels
                 CU(L.rest_list.ensure((size_t)c->kept_cap[t] * 12 + 64));
                 MR.rest_list = L.rest_list.as<uint32_t>();

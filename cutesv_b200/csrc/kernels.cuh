@@ -85,37 +85,45 @@ struct HeadPred {
 
 // Segment step, specialised: the chain-linkage votes of a 2048-element tile are taken with
 // coalesced loads and kept as a bit mask in shared memory (one __ballot_sync per 32 elements);
-// "i starts a cluster of >= min_support members" is then a bit test: link[i] == 0 and
-// link[i+1 .. i+min_support-1] all 1.  Ordered compaction as in k_select.
+// "i starts a cluster of >= min_support members" is then a bit test (core.h chain_head).  Ordered compaction as in
+// k_select.
 static constexpr int HEAD_MAX_NEED_WORDS = 64;  // supports min_support up to ~2000 via the mask; above -> generic path
-// INS / DEL record mode (MR.rec != nullptr): the warps of the CTA then walk the kept clusters whose head lies in the
-// tile and gather ONE 16 B record (+ column c of INS) per member through the input index, written at the member's
-// sorted position -- the cluster kernels read a cluster's members as one contiguous range instead of gathering four
-// or five columns per member.  Only members of kept clusters are touched (a fifth of the filter's survivors on 30x ONT).
+// INS / DEL record mode (MR.rec != nullptr): the tile then gathers ONE 16 B record (+ column c of INS) per member of a kept
+// cluster that lies in it, written at the member's sorted position -- the cluster kernels read a cluster's members as
+// one contiguous range instead of gathering four or five columns per member.  Membership is a bit test too (core.h
+// chain_member, over a backward halo of the mask), so a cluster that crosses a tile edge is gathered by both tiles, and
+// a thread issues the loads of several members before it stores any record.  Only members of kept clusters are touched
+// (a fifth of the filter's survivors on 30x ONT).  The gather is bound by its scattered column loads (one 32 B sector
+// each), not by their latency: DEL takes a from the key where it can.
 struct MemberRec {
     IndelRec* rec; int32_t* recc;
     const int32_t *a, *b, *rid, *c;
     const uint32_t* sidx;
-    // classification of the kept clusters by size while their records are gathered (null: not wanted)
+    // classification of the kept clusters by size (null: not wanted)
     uint2* small_list; uint32_t* n_small;    // (kept ordinal, members) for <= 32 members
     uint32_t* rest_list; uint32_t* n_rest;   // kept ordinal for the others: > REST_SPLIT members from the front,
     uint32_t* n_rest_lo; uint32_t rest_cap;  // ... the others from the end of the rest_cap words
+    // DEL: the contigs' linear offsets (n_contigs + 1).  In a tile that lies on one contig a member's a is its key minus
+    // the contig's offset, so the gather loads one scattered column fewer (null: load every column)
+    const uint64_t* del_off; int n_contigs;
 };
 static constexpr int REST_SPLIT = 64;
+static constexpr int GATHER_GROUP = 4;   // 32 registers per thread (eight CTAs per SM) hold a group of 4 members' loads
 __global__ void __launch_bounds__(SEL_THREADS) k_select_heads(TypeJob J, uint32_t* out, uint32_t out_cap, uint32_t* out_count,
                                                               TileSync ts, uint32_t* status_word, uint32_t overflow_bit, MemberRec MR) {
     pdl_launch_dependents(); pdl_wait();   // programmatic dependent launch: resident early, starts when the previous kernel has finished
     constexpr int WORDS = SEL_TILE / 32;
-    __shared__ uint32_t s_link[WORDS + HEAD_MAX_NEED_WORDS + 2];
+    // mask words: [0, back) before the tile, then the tile's WORDS, then fwd after it
+    __shared__ uint32_t s_link[HEAD_MAX_NEED_WORDS + WORDS + HEAD_MAX_NEED_WORDS];
     __shared__ uint32_t s_warp[9];
-    __shared__ uint32_t s_tile, s_excl;
-    __shared__ uint32_t s_nheads, s_hnext;
-    __shared__ uint16_t s_heads[SEL_TILE];
-    __shared__ uint8_t s_msize[SEL_TILE];   // record mode: members of head h (<= 32), 33: up to REST_SPLIT, 34: more
+    __shared__ uint32_t s_tile, s_excl, s_aoff;
+    __shared__ uint8_t s_msize[SEL_TILE];   // size lists: size class of the tile's h-th head (core.h chain_size_class)
     const int64_t n = job_n(J);
     const uint32_t gen = ts_gen(ts);
     const int need = J.cp.min_support;
-    const int halo_words = (need + 31) / 32 + 1;
+    // record mode reads need - 1 links on both sides of every position, and REST_SPLIT links after a head
+    const int back = MR.rec ? (need + 31) / 32 + 1 : 0;
+    const int fwd = (MR.rec ? max((need + 31) / 32, (REST_SPLIT + 32) / 32) : (need + 31) / 32) + 1;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     while (true) {
         if (threadIdx.x == 0) s_tile = atomicAdd(ts.ticket, 1u);
@@ -123,54 +131,54 @@ __global__ void __launch_bounds__(SEL_THREADS) k_select_heads(TypeJob J, uint32_
         const uint32_t tile = s_tile;
         const int64_t base = (int64_t)tile * SEL_TILE;
         if (base >= n) break;
-        // link bits for [base, base + SEL_TILE + 32*halo_words): votes are evaluated in batches
+        // link bits for [base - 32*back, base + SEL_TILE + 32*fwd): votes are evaluated in batches
         // of 8 words per warp so that the key loads of a batch are all in flight together
-        for (int w0 = warp; w0 < WORDS + halo_words; w0 += 8 * (SEL_THREADS / 32)) {
+        for (int w0 = warp; w0 < back + WORDS + fwd; w0 += 8 * (SEL_THREADS / 32)) {
             bool l[8];
 #pragma unroll
             for (int u = 0; u < 8; u++) {
                 const int w = w0 + u * (SEL_THREADS / 32);
-                const int64_t i = base + (int64_t)w * 32 + lane;
-                l[u] = (w < WORDS + halo_words && i > 0 && i < n) ? job_linked(J, i) : false;
+                const int64_t i = base + (int64_t)(w - back) * 32 + lane;
+                l[u] = (w < back + WORDS + fwd && i > 0 && i < n) ? job_linked(J, i) : false;
             }
 #pragma unroll
             for (int u = 0; u < 8; u++) {
                 const int w = w0 + u * (SEL_THREADS / 32);
                 const uint32_t m = __ballot_sync(0xffffffffu, l[u]);
-                if (lane == 0 && w < WORDS + halo_words) s_link[w] = m;
+                if (lane == 0 && w < back + WORDS + fwd) s_link[w] = m;
             }
         }
+        // DEL: the contig of the tile's first key by a 32-ary search, kept when the tile's last key lies on it too (the last
+        // warp does it: it has the fewest mask words)
+        if (MR.del_off && warp == SEL_THREADS / 32 - 1) {
+            const uint64_t k0 = J.keys32[base], k1 = J.keys32[min(base + SEL_TILE, n) - 1];
+            int lo = 0, span = MR.n_contigs;   // off[lo] <= k0 < off[lo + span]
+            while (span > 1) {
+                const int step = (span + 31) / 32;
+                const bool le = lane * step < span && MR.del_off[lo + lane * step] <= k0;
+                const int j = 31 - __clz(__ballot_sync(0xffffffffu, le));
+                lo += j * step;
+                span = min(step, span - j * step);
+            }
+            if (lane == 0) s_aoff = k1 < MR.del_off[lo + 1] ? (uint32_t)MR.del_off[lo] : ~0u;   // ~0u: it crosses a contig end
+        }
         __syncthreads();
-        const int p0 = threadIdx.x * SEL_ITEMS;
+        const int p0 = threadIdx.x * SEL_ITEMS, q0 = back * 32;   // tile position p is mask bit q0 + p
         uint32_t flags = 0, cnt = 0;
 #pragma unroll
         for (int j = 0; j < SEL_ITEMS; j++) {
             const int p = p0 + j;
-            if (base + p >= n) continue;
-            if (s_link[p >> 5] >> (p & 31) & 1u) continue;   // chained to its predecessor: not a head
-            // bits p+1 .. p+need-1 must all be set
-            int remaining = need - 1, q = p + 1;
-            bool ok = true;
-            while (remaining > 0) {
-                const int wi = q >> 5, bo = q & 31;
-                const int take = min(32 - bo, remaining);
-                const uint32_t mask = (take == 32 ? 0xffffffffu : ((1u << take) - 1u)) << bo;
-                if ((s_link[wi] & mask) != mask) { ok = false; break; }
-                q += take; remaining -= take;
-            }
-            if (ok) { flags |= 1u << j; cnt++; }
+            if (base + p < n && chain_head(s_link, q0 + p, need)) { flags |= 1u << j; cnt++; }
         }
         uint32_t total;
         const uint32_t local = block_excl_scan_256(cnt, s_warp, &total);
-        if (MR.rec) {   // the tile's heads in order; the member gather needs their tile positions, not their ordinals
+        if (MR.small_list) {   // the heads' size classes, in head order
             uint32_t o = local;
 #pragma unroll
             for (int j = 0; j < SEL_ITEMS; j++)
-                if (flags >> j & 1u) s_heads[o++] = (uint16_t)(p0 + j);
-            if (threadIdx.x == 0) { s_nheads = total; s_hnext = 0; }
-            __syncthreads();
+                if (flags >> j & 1u) s_msize[o++] = (uint8_t)chain_size_class(s_link, q0 + p0 + j, REST_SPLIT);
         }
-        // warp 0 waits for the look-back while the other warps gather the members (it joins them afterwards)
+        // warp 0 waits for the look-back while the other warps gather the members (it gathers its share afterwards)
         if (threadIdx.x < 32) {
             const uint32_t ex = lookback_exclusive_warp(ts.status, gen, (int)tile, total);
             if (threadIdx.x == 0) {
@@ -178,43 +186,37 @@ __global__ void __launch_bounds__(SEL_THREADS) k_select_heads(TypeJob J, uint32_
                 if (base + SEL_TILE >= n) *out_count = ex + total;
             }
         }
-        if (MR.rec) {
-            const uint32_t nh = s_nheads;
+        if (MR.rec) {   // positions threadIdx.x + j * SEL_THREADS: every load instruction of a warp reads consecutive words
+            uint32_t mem = 0;
+#pragma unroll 1
+            for (int j = 0; j < SEL_ITEMS; j++) {
+                const int p = threadIdx.x + j * SEL_THREADS;
+                if (base + p < n && chain_member(s_link, q0 + p, need)) mem |= 1u << j;
+            }
+            const uint32_t* __restrict__ sidx = MR.sidx;
+            const int32_t *__restrict__ ca = MR.a, *__restrict__ cb = MR.b, *__restrict__ cr = MR.rid, *__restrict__ cc = MR.c;
+            IndelRec* __restrict__ rec = MR.rec;
+            int32_t* __restrict__ recc = MR.recc;
+            const uint32_t aoff = MR.del_off ? s_aoff : ~0u;
             uint32_t bad = 0;
-            while (true) {
-                uint32_t h = 0;
-                if (lane == 0) h = atomicAdd(&s_hnext, 1u);
-                h = __shfl_sync(0xffffffffu, h, 0);
-                if (h >= nh) break;
-                const int64_t s0 = base + s_heads[h];
-                // members s0 .. s0+m-1: 32 links per step until the first missing one
-                int64_t done = 1;
-                while (true) {
-                    const int64_t i = s0 + done + lane;
-                    const bool brk = (i >= n) || !job_linked(J, i);
-                    const uint32_t bm = __ballot_sync(0xffffffffu, brk);
-                    const int take = bm ? __ffs(bm) - 1 : 32;
-                    if (lane < take) {   // element i is a member
-                        const uint32_t x = MR.sidx[i];
+#pragma unroll 1
+            for (int j0 = 0; j0 < SEL_ITEMS; j0 += GATHER_GROUP) {   // a group's column loads in flight together
+                uint32_t x[GATHER_GROUP];
+#pragma unroll
+                for (int u = 0; u < GATHER_GROUP; u++)
+                    if (mem >> (j0 + u) & 1u) x[u] = sidx[base + threadIdx.x + (j0 + u) * SEL_THREADS];
+#pragma unroll
+                for (int u = 0; u < GATHER_GROUP; u++) {
+                    if (mem >> (j0 + u) & 1u) {
+                        const int64_t i = base + threadIdx.x + (j0 + u) * SEL_THREADS;
                         IndelRec r;
-                        r.a = MR.a[x]; r.b = MR.b[x]; r.rid = MR.rid[x]; r.idx = x;
-                        const int32_t c5 = MR.c ? MR.c[x] : 0;
+                        r.a = aoff != ~0u ? (int32_t)(J.keys32[i] - aoff) : ca[x[u]];
+                        r.b = cb[x[u]]; r.rid = cr[x[u]]; r.idx = x[u];
+                        const int32_t c5 = cc ? cc[x[u]] : 0;
                         if (r.rid < 0 || r.b < 0 || c5 < 0) bad |= ST_NEG_FIELD;
-                        *reinterpret_cast<int4*>(&MR.rec[i]) = *reinterpret_cast<const int4*>(&r);
-                        if (MR.recc) MR.recc[i] = c5;
+                        *reinterpret_cast<int4*>(&rec[i]) = *reinterpret_cast<const int4*>(&r);
+                        if (recc) recc[i] = c5;
                     }
-                    if (bm) { done += take; break; }
-                    done += 32;
-                }
-                if (lane == 0) s_msize[h] = (uint8_t)(done <= 32 ? done : done <= REST_SPLIT ? 33 : 34);
-                if (lane == 0) {   // the head itself
-                    const uint32_t x = MR.sidx[s0];
-                    IndelRec r;
-                    r.a = MR.a[x]; r.b = MR.b[x]; r.rid = MR.rid[x]; r.idx = x;
-                    const int32_t c5 = MR.c ? MR.c[x] : 0;
-                    if (r.rid < 0 || r.b < 0 || c5 < 0) bad |= ST_NEG_FIELD;
-                    *reinterpret_cast<int4*>(&MR.rec[s0]) = *reinterpret_cast<const int4*>(&r);
-                    if (MR.recc) MR.recc[s0] = c5;
                 }
             }
             if (bad) atomicOr(status_word, bad);
@@ -230,10 +232,10 @@ __global__ void __launch_bounds__(SEL_THREADS) k_select_heads(TypeJob J, uint32_
             }
         }
         if (MR.small_list) {   // the size lists of the cluster kernels, one atomic per warp and list; kept ordinal = s_excl + h
-            const uint32_t nh = s_nheads, ex = s_excl;
-            for (uint32_t h0 = warp * 32; h0 < nh; h0 += SEL_THREADS) {
+            const uint32_t ex = s_excl;
+            for (uint32_t h0 = warp * 32; h0 < total; h0 += SEL_THREADS) {
                 const uint32_t h = h0 + lane;
-                const uint32_t sz = h < nh ? s_msize[h] : 255u;
+                const uint32_t sz = h < total ? s_msize[h] : 255u;
                 const uint32_t lt = (1u << lane) - 1u;
                 const uint32_t m_small = __ballot_sync(0xffffffffu, sz <= 32u);
                 const uint32_t m_lo = __ballot_sync(0xffffffffu, sz == 33u), m_hi = __ballot_sync(0xffffffffu, sz == 34u);

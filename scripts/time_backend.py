@@ -8,7 +8,10 @@ Prints, per type:
   * the kept-cluster sizes by route: <= 32 (register kernel), 33-128 (k_cluster_warp), 129-2048 (k_cluster_block in
     shared memory), larger (global scratch), from Engine.counters() of a call of that type alone;
   * the k_select_heads tiles (2048 survivors each) against the CTA slots of one wave: 256 threads and 32 registers per
-    thread (-Xptxas -v) make eight CTAs per SM, and the host launches min(tiles of the signature count, one wave)."""
+    thread (-Xptxas -v) make eight CTAs per SM, and the host launches min(tiles of the signature count, one wave);
+  * the back-end kernels one by one (lanes serialised, CUDA events around every launch): time per launch;
+  * the counts that size the work, per type: density-filter survivors, kept clusters by size class, members and
+    candidates emitted."""
 import json
 import os
 import subprocess
@@ -47,6 +50,14 @@ for _ in range(steps):
 e.fetch()
 kt = e.kernel_times()
 e.set_profiling(False)
+e.set_lanes(False)
+e.set_profiling(True)
+for _ in range(steps):
+    e.cluster_device(mask)
+e.fetch()
+kser = e.kernel_times()
+e.set_profiling(False)
+e.set_lanes(True)
 n_sm = torch.cuda.get_device_properties(0).multi_processor_count
 print("config %d scale %g, %s: %d signatures, %d steps" % (cid, scale, card, cfg["n_sigs"], steps))
 out = {"card": card, "config": cid, "scale": scale}
@@ -61,11 +72,18 @@ for t in types:
     n_sig = len(cfg["sigs"][t]["a"])
     tiles = (surv + SEL_TILE - 1) // SEL_TILE
     ctas = min(max((n_sig + SEL_TILE - 1) // SEL_TILE, 1), SEL_CTAS_PER_SM * n_sm)
-    row = dict(backend_us=1e3 * ms / n if n else None, kept=kept, le32=small, c33_128=kept - small - big, c129_2048=big - giant,
+    row = dict(backend_us=1e3 * ms / n if n else None, candidates=c["n_cand"], kept=kept, le32=small, c33_128=kept - small - big, c129_2048=big - giant,
                gt2048=giant, members=c["members"][t], survivors=surv, select_tiles=tiles, select_ctas=ctas, sms=n_sm)
     out[t] = row
-    print("  %s: filter end -> lane end %s us; kept %d: <=32 %d, 33-128 %d, 129-2048 %d, >2048 %d (members %d); "
+    print("  %s: filter end -> lane end %s us; kept %d: <=32 %d, 33-128 %d, 129-2048 %d, >2048 %d (members %d, candidates %d); "
           "k_select_heads %d tiles of %d survivors, %d CTAs launched (%d SMs)"
           % (t, "%.1f" % row["backend_us"] if n else "n/a (no density filter)", kept, small, row["c33_128"], row["c129_2048"],
-             giant, row["members"], tiles, surv, ctas, n_sm))
+             giant, row["members"], row["candidates"], tiles, surv, ctas, n_sm))
+BACK_END = ("k_part_filter", "k_select_heads", "k_cluster_small", "k_cluster_warp<DEL", "k_cluster_warp<INS", "k_cluster_block<INDEL")
+print("  back-end kernels, lanes serialised (per launch):")
+out["kernels_us"] = {}
+for nm, (n, ms) in sorted(kser.items()):
+    if nm.startswith(BACK_END):
+        out["kernels_us"][nm] = 1e3 * ms / n
+        print("    %-40s launches/step %4.1f  %8.2f us" % (nm, n / steps, 1e3 * ms / n))
 print(json.dumps(out))
