@@ -1129,7 +1129,7 @@ static int run_indel(csv_ctx* c, Lane& L, int t, uint32_t kslot_base) {
         if ((((uintptr_t)s.chrom.p) | ((uintptr_t)s.a.p)) & 15)   // k_part_scatter loads both columns 16 B at a time
             return set_err(CSV_E_STATE, "signature columns are not 16 B aligned");
         uint2* pairs = (uint2*)L.keys_a.p;   // 8 B per signature (ensure_lane_scratch)
-        LAUNCH(c, st, k_part_scatter, n_chunks, 256, ps_smem_bytes(), s.chrom.as<int32_t>(), s.a.as<int32_t>(), n, is_ins, ct, W, P,
+        LAUNCH(c, st, k_part_scatter, n_chunks, PS_THREADS, ps_smem_bytes(), s.chrom.as<int32_t>(), s.a.as<int32_t>(), n, is_ins, ct, W, P,
                n_chunks, rb, pairs, runs, edge, &ctr->status);
         stage_end(c, st, CSV_ST_KEYS);
         stage_begin(c, st, CSV_ST_SORT);

@@ -17,6 +17,40 @@ namespace csv {
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
+// 1-D TMA (cp.async.bulk) into shared memory + mbarrier: a copy's completion is signalled to the barrier in transaction
+// bytes.  bulk_load = the arrival that expects `bytes` + the copy; several copies on one barrier take one
+// mbar_expect_tx for their sum and bulk_copy each.  Sizes and addresses are multiples of 16 B.
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void bulk_copy(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)), "l"(src), "r"(bytes),
+                 "r"(smem_u32(bar))
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_load(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
+    mbar_expect_tx(bar, bytes);
+    bulk_copy(dst, src, bytes, bar);
+}
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+    asm volatile(
+        "{\n"
+        "  .reg .pred p;\n"
+        "WAIT_%=:\n"
+        "  mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
+        "  @!p bra WAIT_%=;\n"
+        "}\n" ::"r"(smem_u32(bar)),
+        "r"(parity)
+        : "memory");
+}
+
 
 static constexpr uint32_t LB_LOCAL = 1u << 30;
 static constexpr uint32_t LB_INCL = 2u << 30;

@@ -31,29 +31,8 @@ static constexpr int EX_SLOT_BYTES = (EX_CHUNK + 4) * 4;  // + 4 ops: chunks sta
 static constexpr int EX_SMEM_BYTES = EX_WARPS * EX_RING * EX_SLOT_BYTES;
 static_assert(EX_SLOT_BYTES % 16 == 0, "bulk copies move multiples of 16 B");
 
-// ---- 1-D TMA (cp.async.bulk) + mbarrier: the CIGAR stream of a record is staged tile by tile into a per-warp shared-memory
-// ring, EX_RING tiles ahead of the scan, by ONE lane; completion is signalled through the slot's mbarrier (transaction bytes).
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void bulk_load(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)), "l"(src), "r"(bytes),
-                 "r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        "  .reg .pred p;\n"
-        "WAIT_%=:\n"
-        "  mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "  @!p bra WAIT_%=;\n"
-        "}\n" ::"r"(smem_u32(bar)),
-        "r"(parity)
-        : "memory");
-}
+// ---- 1-D TMA (cp.async.bulk) + mbarrier (devprims.cuh): the CIGAR stream of a record is staged tile by tile into a per-warp
+// shared-memory ring, EX_RING tiles ahead of the scan, by ONE lane; completion is signalled through the slot's mbarrier.
 
 // the rare per-signature work stays out of the scan loop's instruction stream (instruction cache)
 __device__ __noinline__ void ex_push(const ExtractOut& O, const ReadCtx& RC, const ExtractParams& P, MergeState& S, InsPiece* open_pieces, uint32_t cg,

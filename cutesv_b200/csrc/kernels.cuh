@@ -381,102 +381,126 @@ __host__ __device__ constexpr size_t pf_smem_bytes(int w) {
     return (size_t)(1u << (w - BKT_SHIFT)) * 4 + (size_t)(1u << (w - BKT_SHIFT)) / 32 * 4 + (size_t)PF_STAGE * 8;
 }
 
-// One CTA per round of PART_ROUND rows (round c: rows c * PART_ROUND ..).  The round's (key, row) pairs are grouped by
-// partition in shared memory and written back in place, pairs[c * PART_ROUND + q], with coalesced 16 B stores: partition
-// p of round c is the run [runs[p * n_chunks + c], runs[(p + 1) * n_chunks + c]) of that block (row P of the run table
-// holds the round's row count).  The order inside a partition is irrelevant (k_part_filter orders it), and the filter
-// reads a partition as its list of runs, so no pass has to count the rows of every partition before they are written.
-// A round issues all of its loads (16 B per column and thread, 8 of each) before the first key is formed: the loads are
-// the latency the kernel waits on.  `chrom` and `a` must be 16 B aligned (run_indel checks it); only the last 4-row group
-// of the input is loaded row by row.  Rows in the first or last rb buckets of a partition are counted into edge[p][j]
-// (j < BKT_PAD: the j-th bucket of p; BKT_PAD + j: its j-th bucket from the end), the halo of the neighbours' windows.
-static constexpr int PART_ROUND = 8192, PART_ROUND_V = PART_ROUND / 4 / 256;   // 4-row groups per thread
-static_assert(PART_MAX == 4 * 256 && PART_ROUND < (1 << 14), "k_part_scatter tiling");
-__host__ __device__ constexpr size_t ps_smem_bytes() { return (size_t)PART_ROUND * 8 + (size_t)2 * PART_MAX * 4; }
-__global__ void __launch_bounds__(256) k_part_scatter(const int32_t* __restrict__ chrom, const int32_t* __restrict__ a, int64_t n, int is_ins,
-                                                      ContigTab ct, int W, int P, int n_chunks, int rb, uint2* __restrict__ pairs,
-                                                      uint32_t* __restrict__ runs, uint32_t* __restrict__ edge, uint32_t* status) {
+// One 1024-thread CTA per round of PART_ROUND rows (round c: rows c * PART_ROUND ..), one CTA per SM.  The round's
+// (key, row) pairs are grouped by partition in shared memory and written back in place, pairs[c * PART_ROUND + q], with
+// coalesced 16 B stores: partition p of round c is the run [runs[p * n_chunks + c], runs[(p + 1) * n_chunks + c]) of that
+// block (row P of the run table holds the round's row count).  The order inside a partition is irrelevant (k_part_filter
+// orders it), and the filter reads a partition as its list of runs, so no pass has to count the rows of every partition
+// before they are written.  The larger the round, the longer and fewer the runs the filter walks (config 2: 8.4 M rows of a
+// type, P = 741, about 22 pairs per partition and round).  16384 rows give 513 rounds of a type there, about 3.9 waves of
+// one CTA per SM on 132 SMs; 24576 rows (about 2.6 waves) made both kernels slower (DESIGN §5).
+// The round's `chrom` and `a` come in by two 1-D bulk copies on one mbarrier, into the shared memory that later holds the
+// grouped pairs; `chrom` and `a` must be 16 B aligned (run_indel checks it), and only the rows of the input's last
+// partial 4-row group are loaded row by row.  Every thread then reads its PART_ROUND_V 4-row groups with conflict-free
+// 16 B shared loads and keeps their keys in registers until they are placed.  Rows in the first or last rb buckets of a
+// partition are counted into edge[p][j] (j < BKT_PAD: the j-th bucket of p; BKT_PAD + j: its j-th bucket from the end),
+// the halo of the neighbours' windows.
+static constexpr int PS_THREADS = 1024;
+static constexpr int PART_ROUND = 16384, PART_ROUND_V = PART_ROUND / 4 / PS_THREADS;   // 4-row groups per thread
+__host__ __device__ constexpr size_t ps_smem_bytes() { return (size_t)PART_ROUND * 8 + (size_t)PART_MAX * 4; }
+static_assert(PART_MAX == PS_THREADS && PART_ROUND % (4 * PS_THREADS) == 0, "k_part_scatter tiling: one partition per thread");
+// run offsets, row indices and c * PART_ROUND + offset are 32-bit (n < 2^32); one round must fit an SM's opt-in shared memory
+static_assert(ps_smem_bytes() + 256 <= 227 * 1024, "k_part_scatter: one round per SM");
+__global__ void __launch_bounds__(PS_THREADS, 1) k_part_scatter(const int32_t* __restrict__ chrom, const int32_t* __restrict__ a, int64_t n,
+                                                                int is_ins, ContigTab ct, int W, int P, int n_chunks, int rb,
+                                                                uint2* __restrict__ pairs, uint32_t* __restrict__ runs,
+                                                                uint32_t* __restrict__ edge, uint32_t* status) {
     pdl_launch_dependents();
     extern __shared__ __align__(16) uint32_t s_dyn[];
-    uint2* s_st = reinterpret_cast<uint2*>(s_dyn);   // PART_ROUND pairs, grouped by partition
-    uint32_t* s_off = s_dyn + 2 * PART_ROUND;        // rows of the round per partition -> their first position in s_st
-    uint32_t* s_fill = s_off + PART_MAX;             // next free position of every partition in s_st
-    __shared__ uint32_t s_warp[9];
-    const int64_t s0 = (int64_t)blockIdx.x * PART_ROUND;   // a multiple of 4
+    uint2* s_st = reinterpret_cast<uint2*>(s_dyn);                   // PART_ROUND pairs, grouped by partition
+    int32_t* s_c = reinterpret_cast<int32_t*>(s_dyn);                // before that: the round's chrom ..
+    int32_t* s_a = reinterpret_cast<int32_t*>(s_dyn) + PART_ROUND;   // .. and a
+    uint32_t* s_fill = s_dyn + 2 * PART_ROUND;   // rows of the round per partition -> next free position of it in s_st
+    __shared__ uint32_t s_warp[32];
+    __shared__ __align__(8) uint64_t s_bar;
+    const int t = (int)threadIdx.x, lane = t & 31, warp = t >> 5;
+    const int64_t s0 = (int64_t)blockIdx.x * PART_ROUND;
     const int m = (int)min((int64_t)PART_ROUND, n - s0);
-    for (int p = threadIdx.x; p < PART_MAX; p += 256) s_off[p] = 0;
-    int4 cv[PART_ROUND_V], av[PART_ROUND_V];   // rows s0 + r .. s0 + r + 3, r = 4 * (j * 256 + thread)
-#pragma unroll
-    for (int j = 0; j < PART_ROUND_V; j++) {
-        const int r = 4 * (j * 256 + (int)threadIdx.x);
-        if (r + 4 <= m) {
-            cv[j] = __ldcs(reinterpret_cast<const int4*>(chrom + s0 + r));
-            av[j] = __ldcs(reinterpret_cast<const int4*>(a + s0 + r));
+    const int m4 = m & ~3;   // rows of whole 4-row groups: the bulk copies' share
+    if (t == 0) {
+        mbar_init(&s_bar, 1);
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the barrier init, visible to the async proxy
+        if (m4) {
+            mbar_expect_tx(&s_bar, (uint32_t)m4 * 8);
+            bulk_copy(s_c, chrom + s0, (uint32_t)m4 * 4, &s_bar);
+            bulk_copy(s_a, a + s0, (uint32_t)m4 * 4, &s_bar);
         } else {
-            cv[j] = make_int4(r < m ? chrom[s0 + r] : 0, r + 1 < m ? chrom[s0 + r + 1] : 0, r + 2 < m ? chrom[s0 + r + 2] : 0,
-                              r + 3 < m ? chrom[s0 + r + 3] : 0);
-            av[j] = make_int4(r < m ? a[s0 + r] : 0, r + 1 < m ? a[s0 + r + 1] : 0, r + 2 < m ? a[s0 + r + 2] : 0,
-                              r + 3 < m ? a[s0 + r + 3] : 0);
+            mbar_arrive(&s_bar);
         }
     }
-    uint32_t key[4 * PART_ROUND_V], bad = 0;
+    if (m4 + t < m) { s_c[m4 + t] = chrom[s0 + m4 + t]; s_a[m4 + t] = a[s0 + m4 + t]; }   // the input's last rows
+    s_fill[t] = 0;
+    __syncthreads();   // the barrier initialised; the tail rows and s_fill written
+    mbar_wait(&s_bar, 0);
+    uint32_t key[4 * PART_ROUND_V], bad = 0;   // row 4 * (j * PS_THREADS + thread) + i at key[4 * j + i]
 #pragma unroll
     for (int j = 0; j < PART_ROUND_V; j++) {
-        const int r = 4 * (j * 256 + (int)threadIdx.x);
+        const int r = 4 * (j * PS_THREADS + t);
+        const int4 cv = reinterpret_cast<const int4*>(s_c)[j * PS_THREADS + t];
+        const int4 av = reinterpret_cast<const int4*>(s_a)[j * PS_THREADS + t];
         uint32_t b0 = 0, b1 = 0, b2 = 0, b3 = 0;   // rows past the input are not validated
-        key[4 * j] = indel_key32(cv[j].x, av[j].x, is_ins, ct, b0);
-        key[4 * j + 1] = indel_key32(cv[j].y, av[j].y, is_ins, ct, b1);
-        key[4 * j + 2] = indel_key32(cv[j].z, av[j].z, is_ins, ct, b2);
-        key[4 * j + 3] = indel_key32(cv[j].w, av[j].w, is_ins, ct, b3);
+        key[4 * j] = indel_key32(cv.x, av.x, is_ins, ct, b0);
+        key[4 * j + 1] = indel_key32(cv.y, av.y, is_ins, ct, b1);
+        key[4 * j + 2] = indel_key32(cv.z, av.z, is_ins, ct, b2);
+        key[4 * j + 3] = indel_key32(cv.w, av.w, is_ins, ct, b3);
         bad |= (r < m ? b0 : 0u) | (r + 1 < m ? b1 : 0u) | (r + 2 < m ? b2 : 0u) | (r + 3 < m ? b3 : 0u);
     }
     if (bad) atomicOr(status, bad);
     const uint32_t bmask = (1u << (W - BKT_SHIFT)) - 1;
 #pragma unroll
     for (int k = 0; k < 4 * PART_ROUND_V; k++) {
+        if (4 * ((k >> 2) * PS_THREADS + t) + (k & 3) >= m) continue;
         const uint32_t p = key[k] >> W, bl = (key[k] >> BKT_SHIFT) & bmask;
-        if (4 * ((k >> 2) * 256 + (int)threadIdx.x) + (k & 3) < m && (bl < (uint32_t)rb || bmask - bl < (uint32_t)rb)) {
-            if (bl < (uint32_t)rb) atomicAdd(&edge[p * 2 * BKT_PAD + bl], 1u);
-            if (bmask - bl < (uint32_t)rb) atomicAdd(&edge[p * 2 * BKT_PAD + BKT_PAD + (bmask - bl)], 1u);
-        }
+        if (bl < (uint32_t)rb) atomicAdd(&edge[p * 2 * BKT_PAD + bl], 1u);
+        if (bmask - bl < (uint32_t)rb) atomicAdd(&edge[p * 2 * BKT_PAD + BKT_PAD + (bmask - bl)], 1u);
+        atomicAdd(&s_fill[p], 1u);
     }
-    __syncthreads();   // s_off cleared
+    __syncthreads();   // every row counted, and read: the pairs may now overwrite the input
+    {   // exclusive scan of the per-partition counts, one partition per thread; the run table gets rows 0..P-1
+        const uint32_t v = s_fill[t];
+        uint32_t incl = v;
 #pragma unroll
-    for (int k = 0; k < 4 * PART_ROUND_V; k++)
-        if (4 * ((k >> 2) * 256 + (int)threadIdx.x) + (k & 3) < m) atomicAdd(&s_off[key[k] >> W], 1u);
-    __syncthreads();
-    {   // exclusive scan of the per-partition counts, four partitions per thread; the run table gets rows 0..P-1
-        const uint4 v = reinterpret_cast<const uint4*>(s_off)[threadIdx.x];
-        uint32_t total;
-        const uint32_t ex = block_excl_scan_256(v.x + v.y + v.z + v.w, s_warp, &total);
-        const uint4 o = make_uint4(ex, ex + v.x, ex + v.x + v.y, ex + v.x + v.y + v.z);
-        reinterpret_cast<uint4*>(s_fill)[threadIdx.x] = o;
-        const int p0 = 4 * (int)threadIdx.x;
-        uint32_t* rc = runs + (int64_t)p0 * n_chunks + blockIdx.x;
-        if (p0 < P) rc[0] = o.x;
-        if (p0 + 1 < P) rc[n_chunks] = o.y;
-        if (p0 + 2 < P) rc[2 * (int64_t)n_chunks] = o.z;
-        if (p0 + 3 < P) rc[3 * (int64_t)n_chunks] = o.w;
-        if (threadIdx.x == 0) runs[(int64_t)P * n_chunks + blockIdx.x] = (uint32_t)m;
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint32_t y = __shfl_up_sync(0xffffffffu, incl, d);
+            if (lane >= d) incl += y;
+        }
+        if (lane == 31) s_warp[warp] = incl;
+        __syncthreads();
+        if (warp == 0) {
+            const uint32_t w = s_warp[lane];
+            uint32_t wi = w;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const uint32_t y = __shfl_up_sync(0xffffffffu, wi, d);
+                if (lane >= d) wi += y;
+            }
+            s_warp[lane] = wi - w;
+        }
+        __syncthreads();
+        const uint32_t o = s_warp[warp] + incl - v;
+        s_fill[t] = o;
+        if (t < P) runs[(int64_t)t * n_chunks + blockIdx.x] = o;
+        if (t == 0) runs[(int64_t)P * n_chunks + blockIdx.x] = (uint32_t)m;
     }
     __syncthreads();
 #pragma unroll
     for (int k = 0; k < 4 * PART_ROUND_V; k++) {
-        const int q = 4 * ((k >> 2) * 256 + (int)threadIdx.x) + (k & 3);
+        const int q = 4 * ((k >> 2) * PS_THREADS + t) + (k & 3);
         if (q < m) s_st[atomicAdd(&s_fill[key[k] >> W], 1u)] = make_uint2(key[k], (uint32_t)(s0 + q));
     }
     __syncthreads();
     uint2* dst = pairs + s0;   // 16 B aligned: s0 is a multiple of PART_ROUND
-    for (int q = threadIdx.x; q < (m >> 1); q += 256) reinterpret_cast<uint4*>(dst)[q] = reinterpret_cast<const uint4*>(s_st)[q];
-    if ((m & 1) && threadIdx.x == 0) dst[m - 1] = s_st[m - 1];
+    for (int q = t; q < (m >> 1); q += PS_THREADS) reinterpret_cast<uint4*>(dst)[q] = reinterpret_cast<const uint4*>(s_st)[q];
+    if ((m & 1) && t == 0) dst[m - 1] = s_st[m - 1];
 }
 
 // f(pair, valid) for every pair of partition p, i.e. of the runs [c * PART_ROUND + runs[p][c], c * PART_ROUND +
 // runs[p + 1][c]) of the rounds c < n_chunks (k_part_scatter's run table, runs[p][c] at runs[p * n_chunks + c]).  Every
-// warp takes tiles of 32 consecutive runs, one per lane, in turn with the CTA's other warps (the next tile's run bounds are
-// loaded before the current one is walked).  A warp scan of the run lengths numbers the tile's pairs; the lane that takes
-// pair e finds its run by a five-step binary search over the lanes' run ends (shuffles: no shared memory, no per-pair
-// search in memory).  U pairs per lane are loaded before f sees the first.  f is called by every lane of the warp
+// warp takes tiles of TR consecutive runs, one per lane, in turn with the CTA's other warps (the next tile's run bounds are
+// loaded before the current one is walked).  TR = 32 when every warp gets at least two such tiles, else 16 (lanes TR..31
+// hold empty runs), so that a partition of few runs still spreads over all eight warps.  A warp scan of the run lengths
+// numbers the tile's pairs; the lane that takes pair e finds its run by a five-step binary search over the lanes' run ends
+// (shuffles: no shared memory, no per-pair search in memory).  U pairs per lane are loaded before f sees the first.  f is called by every lane of the warp
 // together, `valid` false past the tile's last pair.
 template <int U, class F>
 __device__ __forceinline__ void part_walk_runs(const uint2* __restrict__ pairs, const uint32_t* __restrict__ runs, int p, int n_chunks,
@@ -484,10 +508,12 @@ __device__ __forceinline__ void part_walk_runs(const uint2* __restrict__ pairs, 
     const int lane = threadIdx.x & 31;
     const uint32_t* r0 = runs + (int64_t)p * n_chunks;
     const uint32_t* r1 = r0 + n_chunks;
-    int c = (int)(threadIdx.x & ~31u) + lane;   // warp w starts at run 32 w
+    const int TR = n_chunks >= 2 * 8 * 32 ? 32 : 16;
+    const bool mine = lane < TR;
+    int c = (int)(threadIdx.x >> 5) * TR + lane;   // warp w starts at run TR w
     uint32_t nb = 0, ne = 0;
-    if (c < n_chunks) { nb = __ldcg(r0 + c); ne = __ldcg(r1 + c); }
-    for (; c - lane < n_chunks; c += 256) {
+    if (mine && c < n_chunks) { nb = __ldcg(r0 + c); ne = __ldcg(r1 + c); }
+    for (; c - lane < n_chunks; c += 8 * TR) {
         const uint32_t len = ne - nb;
         uint32_t end = len;   // inclusive scan of the run lengths: the tile's pairs end[r - 1] .. end[r] - 1 are run r's
 #pragma unroll
@@ -498,7 +524,7 @@ __device__ __forceinline__ void part_walk_runs(const uint2* __restrict__ pairs, 
         const uint32_t tot = __shfl_sync(0xffffffffu, end, 31);
         const uint32_t src = (uint32_t)c * PART_ROUND + nb - (end - len);   // pair e of the tile, in run r: pairs[src(r) + e]
         nb = ne = 0;
-        if (c + 256 < n_chunks) { nb = __ldcg(r0 + c + 256); ne = __ldcg(r1 + c + 256); }
+        if (mine && c + 8 * TR < n_chunks) { nb = __ldcg(r0 + c + 8 * TR); ne = __ldcg(r1 + c + 8 * TR); }
         const uint32_t end15 = __shfl_sync(0xffffffffu, end, 15);   // the searches' first step
         for (uint32_t e0 = 0; e0 < tot; e0 += 32 * U) {
             uint32_t at[U];
@@ -567,7 +593,8 @@ __global__ void __launch_bounds__(256) k_part_filter(const uint2* __restrict__ p
             (right ? s_hr : s_hl)[j] = ok ? edge[(int64_t)q * 2 * BKT_PAD + (right ? 0 : BKT_PAD) + j] : 0u;
         }
         // 1. histogram (the partition's pairs are the runs of the scatter's rounds)
-        constexpr int U = 16;   // loads in flight per thread: a tile of 32 runs (about 360 pairs at W = 22) in one round trip
+        constexpr int U = 16;   // loads in flight per thread: a tile of 32 runs (about 700 pairs at W = 22) in two round trips
+                                // (24 was no faster, DESIGN §5)
         part_walk_runs<U>(pairs, runs, p, n_chunks, [&](uint2 pr, bool v) {
             if (v) atomicAdd(&s_h[phys((pr.x >> BKT_SHIFT) & bmask)], 1u);
         });
