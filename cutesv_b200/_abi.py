@@ -70,6 +70,10 @@ class csv_name_cols(C.Structure):
     _fields_ = [("n_bytes", C.c_int64), ("name_off", _I64P), ("names", _U8P)]
 
 
+class csv_sa_text(C.Structure):
+    _fields_ = [("n_records", C.c_int64), ("n_bytes", C.c_int64), ("text_off", _I64P), ("text", _U8P)]
+
+
 CAND_DTYPE = np.dtype([
     ("svtype", "<i4"), ("chrom", "<i4"), ("pos", "<i4"), ("len", "<i4"), ("support", "<i4"),
     ("cipos", "<i4"), ("cilen", "<i4"), ("search_pos", "<i4"), ("pos2", "<i4"), ("aux", "<i4"),
@@ -253,8 +257,10 @@ def _cai_check(name, v, typestrs, device):
 
 class DevicePacket(tuple):
     """device_packet's result: unpacks as (csv_read_cols, cigar address, n_cigar, csv_sa_cols, csv_seq_cols or None); `names` is
-    the csv_name_cols of a named packet (csv_extract*_named_device), else None."""
+    the csv_name_cols of a named packet (csv_extract*_named_device), else None; `sa_text` the csv_sa_text of a packet that carries
+    its SA:Z tags as text (csv_reduce_sa_device fills sa_off and the csv_sa_cols), else None."""
     names = None
+    sa_text = None
 
 
 def device_packet(packet, device):
@@ -269,31 +275,44 @@ def device_packet(packet, device):
     bases and names), not 1-D or not contiguous; ValueError when host and device arrays are mixed (names on a host packet
     included), an array is on another device than `device`, lengths disagree (n record columns, n + 1 offsets, equal SA
     columns), only one of seq_off / seq4 or of names / name_off is given, or read_id comes with names.
-    Whether the addresses really are device memory of `device` is checked again by the library, the offsets' values on the device."""
+    Whether the addresses really are device memory of `device` is checked again by the library, the offsets' values on the device.
+    A device packet may carry its records' SA:Z values as text instead of sa / sa_off: sa_text (uint8) and sa_text_off (int64, n + 1;
+    record i's value is sa_text[sa_text_off[i]:sa_text_off[i + 1]], no tag prefix, no NUL).  The result's `sa_text` then holds
+    them, and its csv_read_cols::sa_off and csv_sa_cols are empty until csv_reduce_sa_device fills them; ValueError for a packet
+    with both forms, one of sa_text / sa_text_off only, or text on a host packet."""
     sa = packet.get("sa") or {}
     named = packet.get("names") is not None or packet.get("name_off") is not None
+    text = packet.get("sa_text") is not None or packet.get("sa_text_off") is not None
+    if text and (sa or packet.get("sa_off") is not None):
+        raise ValueError("a packet carries sa / sa_off or sa_text / sa_text_off: one or the other")
     arrays = [(f, packet.get(f), ("<i4",)) for f in READ_FIELDS] + [(f, packet.get(f), ("<i8",)) for f in ("cigar_off", "sa_off")]
     arrays += [("cigar", packet.get("cigar"), ("<u4", "<i4"))] + [("sa." + f, sa.get(f), ("<i4",)) for f in SA_FIELDS]
     arrays += [("seq_off", packet.get("seq_off"), ("<i8",)), ("seq4", packet.get("seq4"), ("|u1", "<u1"))]
     arrays += [("name_off", packet.get("name_off"), ("<i8",)), ("names", packet.get("names"), ("|u1", "<u1"))]
+    arrays += [("sa_text_off", packet.get("sa_text_off"), ("<i8",)), ("sa_text", packet.get("sa_text"), ("|u1", "<u1"))]
     present = [(f, v, t) for f, v, t in arrays if v is not None]
     on_dev = {f: is_device_array(v) for f, v, _ in present}
     if not any(on_dev.values()):
         if named:
             raise ValueError("names / name_off are accepted on device packets only (a host packet carries read_id)")
+        if text:
+            raise ValueError("sa_text / sa_text_off are accepted on device packets only (a host packet carries sa / sa_off)")
         return None
     if not all(on_dev.values()):
         raise ValueError("arrays of one packet must be all device or all host arrays: host %s, device %s"
                          % (sorted(f for f, d in on_dev.items() if not d), sorted(f for f, d in on_dev.items() if d)))
     if named and packet.get("read_id") is not None:
         raise ValueError("a named packet carries no read_id: the library numbers its records and ranks their names")
-    missing = [f for f, v, _ in arrays[:len(READ_FIELDS) + 3 + len(SA_FIELDS)] if v is None and not (named and f == "read_id")]
+    missing = [f for f, v, _ in arrays[:len(READ_FIELDS) + 3 + len(SA_FIELDS)]
+               if v is None and not (named and f == "read_id") and not (text and (f == "sa_off" or f.startswith("sa.")))]
     if missing:
         raise ValueError("packet arrays missing: %s" % missing)
     if (packet.get("seq_off") is None) != (packet.get("seq4") is None):
         raise ValueError("seq_off and seq4 go together: give both or neither")
     if (packet.get("name_off") is None) != (packet.get("names") is None):
         raise ValueError("name_off and names go together: give both or neither")
+    if (packet.get("sa_text_off") is None) != (packet.get("sa_text") is None):
+        raise ValueError("sa_text_off and sa_text go together: give both or neither")
     ptrs, lens = {}, {}
     for f, v, t in present:
         ptrs[f], lens[f] = _cai_check(f, v, t, device)
@@ -302,11 +321,11 @@ def device_packet(packet, device):
     for f in rfields:
         if lens[f] != n:
             raise ValueError("column lengths disagree: %s" % {g: lens[g] for g in rfields})
-    for f in ("cigar_off", "sa_off") + tuple(f for f in ("seq_off", "name_off") if f in lens):
+    for f in ("cigar_off", "sa_text_off" if text else "sa_off") + tuple(f for f in ("seq_off", "name_off") if f in lens):
         if lens[f] != n + 1:
             raise ValueError("%s has %d entries, expected n + 1 = %d" % (f, lens[f], n + 1))
-    n_sa = lens["sa.chrom"]
-    if any(lens["sa." + f] != n_sa for f in SA_FIELDS):
+    n_sa = 0 if text else lens["sa.chrom"]
+    if not text and any(lens["sa." + f] != n_sa for f in SA_FIELDS):
         raise ValueError("SA column lengths disagree: %s" % {f: lens["sa." + f] for f in SA_FIELDS})
 
     def p(f, ctype=_I32P):
@@ -319,6 +338,8 @@ def device_packet(packet, device):
     out = DevicePacket((reads, C.cast(C.c_void_p(ptrs["cigar"]), _U32P), lens["cigar"], sa_cols, seq))
     if named:
         out.names = csv_name_cols(lens["names"], p("name_off", _I64P), p("names", _U8P))
+    if text:
+        out.sa_text = csv_sa_text(n, lens["sa_text"], p("sa_text_off", _I64P), p("sa_text", _U8P))
     return out
 
 

@@ -70,6 +70,8 @@ _SIGNATURES = {
     "csv_set_scan_regions": (C.c_int, [_VP, C.c_int32, _I64P, C.POINTER(C.c_double), _I64P, _I64P]),
     "csv_scan_append_named_device": (C.c_int, [_VP, C.POINTER(_abi.csv_read_cols), C.POINTER(C.c_uint32), C.c_int64, C.POINTER(_abi.csv_sa_cols),
                                                C.POINTER(_abi.csv_seq_cols), C.POINTER(_abi.csv_name_cols), C.c_int, _VP, _I64P, _I64P, _I64P]),
+    "csv_set_contig_names": (C.c_int, [_VP, C.c_int32, C.POINTER(C.c_uint8), _I64P]),
+    "csv_reduce_sa_device": (C.c_int, [_VP, C.POINTER(_abi.csv_sa_text), _VP, C.POINTER(_I64P), C.POINTER(_abi.csv_sa_cols)]),
     "csv_ins_seq_device_ptrs": (C.c_int, [_VP, C.POINTER(_VP), C.POINTER(_VP), C.POINTER(_VP), _I64P]),
     "csv_fetch_ins_seqs": (C.c_int, [_VP, _I64P, C.c_int64, C.POINTER(C.c_uint8), C.c_int64, _I64P]),
     "csv_extract_reset": (C.c_int, [_VP]),

@@ -24,6 +24,7 @@
 #include "radix.cuh"
 #include "extract.cuh"
 #include "scan_core.h"
+#include "sa_core.h"
 
 using namespace csv;
 
@@ -146,6 +147,15 @@ struct ExtractState {
     double per_record[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // largest yield of a packet so far: signatures per type [0..4], pieces [5] per alignment record
 };
 
+// SA:Z text reduced on the device (sa_api.inl): csv_set_contig_names' table (names sorted bytewise, their contig ids) and the
+// outputs of csv_reduce_sa_device in two sets, so that a call that fails leaves the previous outputs as they were
+struct SaState {
+    DBuf name_bytes, name_off, name_id, cnt;
+    int64_t n_names = 0;             // 0: no table
+    DBuf off[2], col[2][7];          // sa_off and the seven csv_sa_cols columns of each set
+    int cur = 0;                     // the set of the last successful call
+};
+
 // Lanes: SV types are independent until the `order` stage, so their kernel chains run concurrently on
 // separate streams, one lane per SV type (lane t runs type t; lane 0's stream is the ctx stream).  With lanes off every type
 // runs on lane 0.  A lane owns its stream's launch state and the scratch its chain mutates; the chain's functions take it as
@@ -266,6 +276,7 @@ struct csv_ctx {
     uint32_t last_mask = 0x1f;
     // extraction
     ExtractState ex;
+    SaState sa;
     // CUDA graph of one csv_cluster call (kernel chain of all lanes), keyed by everything the enqueue depends on
     struct GraphKey {
         uint32_t mask; int64_t n[CSV_NTYPES]; int64_t n_reads, n_aln; csv_params P; int lanes; uint64_t alloc_epoch; uint64_t cfg_epoch;
@@ -595,6 +606,7 @@ extern "C" int csv_set_contigs(csv_ctx* c, int32_t n, const int64_t* lens) {
     CU(cudaSetDevice(c->device));
     if (c->off_pad == 0) csv_set_params(c, &c->P);
     if ((int32_t)c->owned.size() != n) c->owned.clear();   // a new table drops the shard mask
+    if (c->sa.n_names != n) c->sa.n_names = 0;             // ... and the contig names
     std::vector<int64_t> keep(lens, lens + n);   // (lens may alias c->contig_len)
     c->n_contigs = n;
     c->contig_len = keep;
@@ -1768,3 +1780,4 @@ static int scan_install_alignments(csv_ctx* c, cudaStream_t st, LbPool& lb);
 #include "sigsort_api.inl"
 #include "names_api.inl"
 #include "scan_api.inl"
+#include "sa_api.inl"

@@ -39,10 +39,19 @@ class Engine(object):
         self.params = params
         _lib.check(self.L.csv_set_params(self.h, C.byref(params)))
 
-    def set_contigs(self, lens):
+    def set_contigs(self, lens, names=None):
+        """Contig table (csv_set_contigs); names (str or bytes per contig id, optional): the contig names that SA:Z text reduced on
+        the device (reduce_sa, packets with sa_text) is matched against (csv_set_contig_names)."""
         lens = np.ascontiguousarray(lens, dtype=np.int64)
         self.n_contigs = len(lens)
         _lib.check(self.L.csv_set_contigs(self.h, C.c_int32(len(lens)), lens.ctypes.data_as(C.POINTER(C.c_int64))))
+        if names is not None:
+            enc = [nm.encode() if isinstance(nm, str) else bytes(nm) for nm in names]
+            off = np.zeros(len(enc) + 1, dtype=np.int64)
+            np.cumsum([len(b) for b in enc], out=off[1:])
+            raw = np.frombuffer(b"".join(enc) or b"\0", dtype=np.uint8)
+            _lib.check(self.L.csv_set_contig_names(self.h, C.c_int32(len(enc)), raw.ctypes.data_as(C.POINTER(C.c_uint8)),
+                                                   off.ctypes.data_as(C.POINTER(C.c_int64))))
 
     def set_profiling(self, on):
         """True: every launch between CUDA events.  "lanes": only the INS / DEL back-end intervals and the
@@ -440,13 +449,15 @@ class Engine(object):
         sequences are built on the device (fetch_ins_seqs, ins_seq_tensors).  Device and host packets may be mixed in one
         append accumulation.  A device packet with names / name_off (the records' read names as bytes, instead of read_id) goes
         through csv_extract*_named_device: every packet of the accumulation then carries names, and rank_names() turns the
-        provisional ids (record indices) into name ranks."""
+        provisional ids (record indices) into name ranks.  A device packet with sa_text / sa_text_off (the records' SA:Z values as
+        text) has them reduced on the device first (reduce_sa; needs set_contigs(..., names))."""
         counts = (C.c_int64 * _abi.CSV_NTYPES)()
         n_rows = C.c_int64(0)
         d = _abi.device_packet(packed, self.device)
         if d is not None:
             rc_, cig_p, n_cig, sa_, seq = d
             st = self._producer_stream(stream, [packed])
+            self._reduce_packet_sa(d, st)
             seq_p = C.byref(seq) if seq is not None else None
             if d.names is not None:
                 fn = self.L.csv_extract_append_named_device if append else self.L.csv_extract_named_device
@@ -497,6 +508,38 @@ class Engine(object):
                                                win_start.ctypes.data_as(C.POINTER(C.c_double)), reg_off.ctypes.data_as(C.POINTER(C.c_int64)),
                                                reg.ctypes.data_as(C.POINTER(C.c_int64))))
 
+    def _reduce_sa_call(self, text, stream):
+        """csv_reduce_sa_device on a csv_sa_text: (sa_off address, filled csv_sa_cols)."""
+        off_p, cols = C.POINTER(C.c_int64)(), _abi.csv_sa_cols()
+        _lib.check(self.L.csv_reduce_sa_device(self.h, C.byref(text), C.c_void_p(stream or None), C.byref(off_p), C.byref(cols)))
+        return off_p, cols
+
+    def _reduce_packet_sa(self, d, stream):
+        """A DevicePacket with SA text: its csv_read_cols::sa_off and csv_sa_cols become csv_reduce_sa_device's outputs."""
+        if d.sa_text is None:
+            return
+        off_p, cols = self._reduce_sa_call(d.sa_text, stream)
+        d[0].sa_off = off_p
+        C.memmove(C.addressof(d[3]), C.addressof(cols), C.sizeof(cols))
+
+    def reduce_sa(self, text, text_off, stream=None):
+        """SA:Z values reduced on the device (csv_reduce_sa_device): text (uint8) and text_off (int64, n + 1) torch CUDA tensors, record
+        i's value text[text_off[i]:text_off[i + 1]] without tag prefix or NUL, matched against set_contigs(..., names).  Returns
+        zero-copy torch views (sa_off int64 [n + 1], dict of the seven int32 csv_sa_cols columns, _abi.SA_FIELDS), the sa_off / sa of
+        a device packet.  They are library memory, valid until the next reduce_sa (or a packet with sa_text), set_contigs with names
+        or close(), so clone() what you keep."""
+        import torch
+        to, n1 = _abi._cai_check("sa_text_off", text_off, ("<i8",), self.device)
+        tp, nb = _abi._cai_check("sa_text", text, ("|u1", "<u1"), self.device)
+        if n1 < 1:
+            raise ValueError("sa_text_off needs n + 1 >= 1 entries")
+        t = _abi.csv_sa_text(n1 - 1, nb, C.cast(C.c_void_p(to), C.POINTER(C.c_int64)), C.cast(C.c_void_p(tp), C.POINTER(C.c_uint8)))
+        off_p, cols = self._reduce_sa_call(t, self._producer_stream(stream, [{"t": text, "o": text_off}]))
+        dev = torch.device("cuda", self.device)
+        off = torch.as_tensor(_DeviceView(C.cast(off_p, C.c_void_p).value, (n1,), "<i8"), device=dev)
+        return off, {f: torch.as_tensor(_DeviceView(C.cast(getattr(cols, f), C.c_void_p).value, (cols.n,)), device=dev)
+                     for f in _abi.SA_FIELDS}
+
     def fetch_alignments(self):
         """D2H of csv_cluster's alignment table (upload_alignments, or installed by rank_names after scan(..., alignments=True)):
         dict(chrom, start, end, read_id, is_primary) in the table's order, or None when there is none."""
@@ -518,12 +561,14 @@ class Engine(object):
         no read_id (_abi.scan_packet).  The library drops what the reference's single_pipe drops (no CIGAR, contig < 0, flag 256 or
         272, outside the set_scan_regions table) and extracts the rest in place; alignments=True also keeps every record with a CIGAR
         and a contig as a row of the TRA genotyper's alignment table, which rank_names() installs.  Record numbers (provisional ids,
-        name_rank_tensor, fetch_records, INS pieces) count all scanned records.  Returns extract()'s dict plus n_aln_rows."""
+        name_rank_tensor, fetch_records, INS pieces) count all scanned records.  A packet may carry sa_text / sa_text_off instead of
+        sa / sa_off, reduced on the device first as extract() does.  Returns extract()'s dict plus n_aln_rows."""
         d = _abi.scan_packet(packet, self.device)
         rc_, cig_p, n_cig, sa_, seq = d
         counts = (C.c_int64 * _abi.CSV_NTYPES)()
         n_rows, n_aln = C.c_int64(0), C.c_int64(0)
         st = self._producer_stream(stream, [packet])
+        self._reduce_packet_sa(d, st)
         _lib.check(self.L.csv_scan_append_named_device(self.h, C.byref(rc_), cig_p, C.c_int64(n_cig), C.byref(sa_),
                                                        C.byref(seq) if seq is not None else None, C.byref(d.names), int(bool(alignments)),
                                                        C.c_void_p(st or None), counts, C.byref(n_rows), C.byref(n_aln)))

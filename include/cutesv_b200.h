@@ -488,6 +488,35 @@ int csv_scan_append_named_device(csv_ctx* ctx, const csv_read_cols* reads, const
 int csv_fetch_alignments(csv_ctx* ctx, int64_t cap, int32_t* chrom, int32_t* start, int32_t* end, int32_t* read_id, uint8_t* is_primary,
                          int64_t* n_rows);
 
+/* ---- SA:Z tags reduced on the device ----
+ * The contig names of the csv_set_contigs table, host arrays: name k (contig id k) is names[name_off[k], name_off[k + 1]),
+ * bytes without NUL.  n must equal the table's contig count; names must be non-empty and unique.  Anything else is
+ * CSV_E_INVALID, changing nothing.  The library keeps them sorted bytewise on the device with their ids; a later
+ * csv_set_contigs with another contig count drops them.  Ends the outputs of csv_reduce_sa_device. */
+int csv_set_contig_names(csv_ctx* ctx, int32_t n, const uint8_t* names, const int64_t* name_off);
+
+/* Record i's SA:Z value is text[text_off[i], text_off[i + 1]) (device memory): no tag prefix, no NUL terminator; an empty
+ * range is a record without the tag. */
+typedef struct csv_sa_text {
+    int64_t n_records;
+    int64_t n_bytes;
+    const int64_t* text_off;   /* n_records + 1 */
+    const uint8_t* text;
+} csv_sa_text;
+/* SA:Z text -> the SA table of a device packet: *sa_off (n_records + 1 entries, for csv_read_cols::sa_off) and *sa (the seven
+ * columns, sa->n rows), ctx-owned device memory that csv_extract*_device and csv_scan_append_named_device take as they are.
+ * Valid until the next csv_reduce_sa_device, csv_set_contig_names or csv_destroy; a call that fails leaves them as they were.
+ * The reduction is that of the native BAM decoder (bam_reader.cpp): entries end at ';' (an entry without it is dropped with
+ * everything after it), a NUL byte ends the value, entries of fewer than 5 comma-separated fields are skipped, an unknown
+ * contig name gives contig -1, pos0 = atoi(pos) - 1, strand '+' -> 0 else 1, mapq = atoi(mapq), and the clips and span of
+ * the CIGAR as acquire_clip_pos (cuteSV:466-481) computes them.  Ordered after the caller's work on `stream` (0: the legacy
+ * default stream); the call returns when the outputs are complete.
+ *   - CSV_E_STATE before csv_set_contig_names; CSV_E_INVALID for host memory or null pointers.
+ *   - CSV_E_INPUT, changing nothing: text_off does not start at >= 0, decreases or ends past n_bytes (checked on the
+ *     device); a position, mapq or CIGAR number (or span) whose value does not fit int32.
+ *   - CSV_E_CAPACITY: 2^32 or more entries in one call. */
+int csv_reduce_sa_device(csv_ctx* ctx, const csv_sa_text* text, void* stream, const int64_t** sa_off, csv_sa_cols* sa);
+
 /* Records whose split-read analysis was skipped because they carry more than 64 qualifying segments (only reachable
  * with --max_split_parts -1; their CIGAR signatures are taken).  The reference has no such limit: a documented,
  * counted deviation instead of a failed run. */
