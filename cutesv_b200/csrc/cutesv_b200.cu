@@ -1532,8 +1532,8 @@ extern "C" int csv_cluster(csv_ctx* c, uint32_t type_mask) {
     int rc = ensure_workspace(c, type_mask);
     if (rc) return rc;
     c->gathered = false;
-    // look-back generations are epoch * LB_ORDINALS + ordinal in 32 bits: start over long before they could wrap
-    if (++c->epoch_host >= (1u << 21)) {
+    // look-back generations are epoch * LB_ORDINALS + ordinal in 31 bits: start over before they could wrap
+    if (++c->epoch_host >= LB_EPOCH_LIMIT) {
         CU(cudaDeviceSynchronize());
         CU(cudaMemset(c->d_epoch.p, 0, 64));
         for (Lane& L : c->lanes) if (L.lb_status.p) CU(cudaMemset(L.lb_status.p, 0, L.lb_status.cap));

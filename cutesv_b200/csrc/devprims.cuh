@@ -52,14 +52,18 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 
 
-static constexpr uint32_t LB_LOCAL = 1u << 30;
-static constexpr uint32_t LB_INCL = 2u << 30;
-static constexpr uint32_t LB_MASK = (1u << 30) - 1;
-
-// Status words are 64-bit: [generation:32][flag:2][value:30].  Every launch that uses the
-// look-back gets a fresh generation number from the host, so the status buffer never has to be
-// cleared: words of older generations simply read as "not published yet".
-__device__ __forceinline__ uint64_t lb_word(uint32_t gen, uint32_t flag_value) { return ((uint64_t)gen << 32) | flag_value; }
+// Status words are 64-bit: [generation:31][inclusive:1][value:32].  A word is published when its generation is the
+// launch's; the value is the tile's own total (inclusive = 0) or the sum over tiles 0..tile (inclusive = 1), so a tile
+// total or a prefix may take all 32 bits (sums wrap modulo 2^32, as the scans' uint32 outputs do).  Every launch that uses
+// the look-back gets a fresh generation in [1, LB_GEN_LIMIT), so the status buffer never has to be cleared: words of other
+// generations, and zeroed words (generation 0, never issued), read as "not published yet".
+static constexpr uint32_t LB_GEN_LIMIT = 1u << 31;
+__device__ __forceinline__ uint64_t lb_word(uint32_t gen, bool inclusive, uint32_t value) {
+    return ((uint64_t)gen << 33) | ((uint64_t)inclusive << 32) | value;
+}
+__device__ __forceinline__ bool lb_ready(uint64_t v, uint32_t gen) { return (uint32_t)(v >> 33) == gen; }
+__device__ __forceinline__ bool lb_inclusive(uint64_t v) { return (v >> 32) & 1u; }
+__device__ __forceinline__ uint32_t lb_value(uint64_t v) { return (uint32_t)v; }
 // gpu-scope relaxed accesses: coherent at L2, no L1 caching, cheaper than volatile (.sys)
 __device__ __forceinline__ uint64_t lb_load(const uint64_t* p) {
     uint64_t v;
@@ -69,12 +73,11 @@ __device__ __forceinline__ uint64_t lb_load(const uint64_t* p) {
 __device__ __forceinline__ void lb_store(uint64_t* p, uint64_t v) {
     asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
-__device__ __forceinline__ bool lb_ready(uint64_t v, uint32_t gen) { return (uint32_t)(v >> 32) == gen && (((uint32_t)v) >> 30) != 0; }
 
 // Publishes `local` for `tile` (one thread calls it); lookback_wait_warp later returns the tile's exclusive prefix.
 // Splitting the two lets a CTA do other work while its predecessors publish.
 __device__ __forceinline__ void lookback_publish(uint64_t* status, uint32_t gen, int tile, uint32_t local) {
-    lb_store(status + tile, lb_word(gen, local | (tile == 0 ? LB_INCL : LB_LOCAL)));
+    lb_store(status + tile, lb_word(gen, tile == 0, local));
 }
 
 // Warp-cooperative wait (all 32 lanes of ONE warp call it) after lookback_publish(status, gen, tile, local): returns
@@ -87,23 +90,22 @@ __device__ __forceinline__ uint32_t lookback_wait_warp(uint64_t* status, uint32_
     int p = tile - 1;
     while (true) {
         const int q = p - lane;
-        const uint64_t v = q >= 0 ? lb_load(status + q) : lb_word(gen, LB_INCL);
-        const uint32_t w = (uint32_t)v;
+        const uint64_t v = q >= 0 ? lb_load(status + q) : lb_word(gen, true, 0u);   // before tile 0: an inclusive zero
         const bool ready = lb_ready(v, gen);
         const uint32_t nr = __ballot_sync(0xffffffffu, !ready);
-        const uint32_t inc = __ballot_sync(0xffffffffu, ready && (w >> 30) == 2);
+        const uint32_t inc = __ballot_sync(0xffffffffu, ready && lb_inclusive(v));
         const int first_nr = nr ? __ffs(nr) - 1 : 32;
         const int first_inc = inc ? __ffs(inc) - 1 : 32;
         const bool done = first_inc < first_nr;
         const int upto = done ? first_inc + 1 : first_nr;  // lanes [0, upto) are consumed
-        uint32_t contrib = lane < upto ? (w & LB_MASK) : 0u;
+        uint32_t contrib = lane < upto ? lb_value(v) : 0u;
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) contrib += __shfl_xor_sync(0xffffffffu, contrib, o);
         excl += contrib;
         if (done) break;
         p -= upto;  // upto == 0: the nearest predecessor has not published yet -> poll again
     }
-    if (lane == 0) lb_store(status + tile, lb_word(gen, (excl + local) | LB_INCL));
+    if (lane == 0) lb_store(status + tile, lb_word(gen, true, excl + local));
     return excl;
 }
 
@@ -183,6 +185,9 @@ struct TileSync {
     uint32_t ordinal;        // unique per look-back launch inside one call (< LB_ORDINALS)
 };
 static constexpr uint32_t LB_ORDINALS = 1024;
+// csv_cluster starts its device epoch over before it reaches LB_EPOCH_LIMIT, so that every generation fits 31 bits
+static constexpr uint32_t LB_EPOCH_LIMIT = 1u << 21;
+static_assert((uint64_t)LB_EPOCH_LIMIT * LB_ORDINALS <= LB_GEN_LIMIT, "look-back generations must fit 31 bits");
 // first node of every csv_cluster call: fresh look-back generation, zeroed ticket words and counters (one launch
 // instead of a kernel and two memsets)
 __global__ void __launch_bounds__(256) k_begin(uint32_t* epoch, uint32_t* tickets, int n_tickets, uint32_t* counters, int n_counters,

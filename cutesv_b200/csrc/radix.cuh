@@ -149,9 +149,9 @@ __global__ void __launch_bounds__(RS_THREADS, 4) k_rs_onesweep(const K* __restri
         uint64_t* st = status + d;
         uint32_t excl_tiles = 0;
         if (tile == 0) {
-            lb_store(st, lb_word(gen, sum | LB_INCL));
+            lb_store(st, lb_word(gen, true, sum));
         } else {
-            lb_store(st + (size_t)tile * 256, lb_word(gen, sum | LB_LOCAL));
+            lb_store(st + (size_t)tile * 256, lb_word(gen, false, sum));
             constexpr int LB_BATCH = 8;
             int p = tile - 1;
             bool done = false;
@@ -160,21 +160,20 @@ __global__ void __launch_bounds__(RS_THREADS, 4) k_rs_onesweep(const K* __restri
 #pragma unroll
                 for (int j = 0; j < LB_BATCH; j++) {
                     const int q = p - j;
-                    v[j] = q >= 0 ? lb_load(st + (size_t)q * 256) : lb_word(gen, LB_INCL);
+                    v[j] = q >= 0 ? lb_load(st + (size_t)q * 256) : lb_word(gen, true, 0u);
                 }
                 int used = 0;
 #pragma unroll
                 for (int j = 0; j < LB_BATCH; j++) {
                     if (!done && used == j && lb_ready(v[j], gen)) {
-                        const uint32_t w = (uint32_t)v[j];
-                        excl_tiles += w & LB_MASK;
+                        excl_tiles += lb_value(v[j]);
                         used = j + 1;
-                        if ((w >> 30) == 2) done = true;
+                        if (lb_inclusive(v[j])) done = true;
                     }
                 }
                 p -= used;  // used == 0: nearest predecessor not published yet -> poll again
             }
-            lb_store(st + (size_t)tile * 256, lb_word(gen, (excl_tiles + sum) | LB_INCL));
+            lb_store(st + (size_t)tile * 256, lb_word(gen, true, excl_tiles + sum));
         }
         s_dst[d] = (int64_t)gbase[d] + (int64_t)excl_tiles - (int64_t)excl_local;
     }
