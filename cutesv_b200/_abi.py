@@ -85,7 +85,8 @@ GENO_DTYPE = np.dtype([
     ("status", "<i4"), ("qual", "<f8"),
 ])
 WINDOW_DTYPE = np.dtype([("chrom", "<i4"), ("reserved", "<i4"), ("s2", "<i8"), ("e2", "<i8")])   # csv_window, half units
-assert CAND_DTYPE.itemsize == 64 and GENO_DTYPE.itemsize == 40 and WINDOW_DTYPE.itemsize == 24
+TRA_QUERY_DTYPE = np.dtype([("chr1", "<i4"), ("chr2", "<i4"), ("pos1", "<i8"), ("pos2", "<i8")])   # csv_tra_query
+assert CAND_DTYPE.itemsize == 64 and GENO_DTYPE.itemsize == 40 and WINDOW_DTYPE.itemsize == 24 and TRA_QUERY_DTYPE.itemsize == 24
 
 
 def make_windows(chrom, s2, e2):

@@ -49,6 +49,7 @@ _SIGNATURES = {
     "csv_overlap_cover": (C.c_int, [_VP, _VP, C.c_int64, C.POINTER(_abi.csv_reads_cols), _I32P, _I32P, _I64P, _I32P, C.c_int64, _I64P, _I32P,
                                     C.c_int64, _I64P, _I64P]),
     "csv_call_gt": (C.c_int, [_VP, _VP, C.c_int64, C.c_int32, C.POINTER(_abi.csv_reads_cols), _I64P, _I32P, _VP]),
+    "csv_tra_call_gt": (C.c_int, [_VP, _VP, C.c_int64, C.POINTER(_abi.csv_reads_cols), C.c_int32, C.c_int32, _I64P, _I32P, _VP]),
     "csv_extract": (C.c_int, [_VP, C.POINTER(_abi.csv_read_cols), C.POINTER(C.c_uint32), C.c_int64,
                               C.POINTER(_abi.csv_sa_cols), _I64P, _I64P]),
     "csv_extract_append": (C.c_int, [_VP, C.POINTER(_abi.csv_read_cols), C.POINTER(C.c_uint32), C.c_int64,

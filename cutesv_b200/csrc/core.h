@@ -1144,29 +1144,50 @@ CSV_HD int tra_count_coverage(const AlnView& A, int32_t chr, int64_t s, int64_t 
     }
     return 0;
 }
-// Fills g for one TRA candidate.  sup: its supporting read ids (ascending).
-CSV_HD void tra_call_gt(const AlnView& A, const csv_cand& c, const int32_t* sup, int32_t bias, int32_t gt_round, const csv_geno* gl_table,
-                        csv_geno* g) {
-    const int32_t chr1 = c.chrom, chr2 = c.aux >> 2;
-    const int32_t n_sup = c.names_cnt;
+// The call_gt window of a breakpoint: [max(pos - bias, 0), min(pos + bias, contig length)] (resolveTRA.py:264-265, 292-293)
+CSV_HD void tra_window(const AlnView& A, int32_t chr, int64_t pos, int32_t bias, int64_t* s, int64_t* e) {
+    *s = pos - bias; if (*s < 0) *s = 0;
+    *e = pos + bias; if (*e > A.contig_len[chr]) *e = A.contig_len[chr];
+}
+// call_gt of one breakpoint pair.  sup: the n_sup supporting read ids (ascending, duplicates allowed; DV = n_sup).
+// CC runs count_coverage: TraCountCoverage below for the host, the warp-cooperative scan in kernels.cuh for the device.
+template <class CC>
+CSV_HD csv_geno tra_call_gt_rules(const CC& cc, const AlnView& A, int32_t chr1, int64_t pos1, int32_t chr2, int64_t pos2, const int32_t* sup,
+                                  int32_t n_sup, int32_t bias, int32_t gt_round, const csv_geno* gl_table) {
     const int32_t up = threshold_ref_count(n_sup);
     int32_t nset = 0, dr = 0;
-    int64_t s = (int64_t)c.pos - bias; if (s < 0) s = 0;
-    int64_t e = (int64_t)c.pos + bias; if (e > A.contig_len[chr1]) e = A.contig_len[chr1];
-    const int st = tra_count_coverage(A, chr1, s, e, sup, n_sup, up, gt_round, &nset, &dr, 1, 0);
-    const int64_t s1 = s, e1 = e;
+    int64_t s, e;
+    tra_window(A, chr1, pos1, bias, &s, &e);
+    const int st = cc(A, chr1, s, e, sup, n_sup, up, gt_round, &nset, &dr, 1, 0);
+    csv_geno g;
     if (st == -1) {  // DR '.', GT './.' (resolveTRA.py:277-282)
-        g->dr = -1; g->dv = n_sup; g->gt = -1; g->pl[0] = g->pl[1] = g->pl[2] = 0; g->gq = 0; g->status = 2; g->qual = 0.0;
-        return;
+        g.dr = -1; g.dv = n_sup; g.gt = -1; g.pl[0] = g.pl[1] = g.pl[2] = 0; g.gq = 0; g.status = 2; g.qual = 0.0;
+        return g;
     }
-    if (st == 0) {
-        s = (int64_t)c.pos2 - bias; if (s < 0) s = 0;
-        e = (int64_t)c.pos2 + bias; if (e > A.contig_len[chr2]) e = A.contig_len[chr2];
-        if (chr2 == chr1) tra_count_coverage(A, chr2, s, e, sup, n_sup, up, gt_round, &nset, &dr, s1, e1);
-        else tra_count_coverage(A, chr2, s, e, sup, n_sup, up, gt_round, &nset, &dr, 1, 0);
+    if (st == 0) {  // the second window's status is not used (resolveTRA.py:301)
+        const int64_t s1 = s, e1 = e;
+        tra_window(A, chr2, pos2, bias, &s, &e);
+        if (chr2 == chr1) cc(A, chr2, s, e, sup, n_sup, up, gt_round, &nset, &dr, s1, e1);
+        else cc(A, chr2, s, e, sup, n_sup, up, gt_round, &nset, &dr, 1, 0);
     }
-    *g = gl_table[gl_index(dr, n_sup)];
-    g->dr = dr; g->dv = n_sup;
+    g = gl_table[gl_index(dr, n_sup)];
+    g.dr = dr; g.dv = n_sup;
+    return g;
+}
+struct TraCountCoverage {
+    CSV_HD int operator()(const AlnView& A, int32_t chr, int64_t s, int64_t e, const int32_t* sup, int n_sup, int32_t up_bound, int32_t itround,
+                          int32_t* nset, int32_t* dr, int64_t xs, int64_t xe) const {
+        return tra_count_coverage(A, chr, s, e, sup, n_sup, up_bound, itround, nset, dr, xs, xe);
+    }
+};
+CSV_HD csv_geno tra_call_gt(const AlnView& A, int32_t chr1, int64_t pos1, int32_t chr2, int64_t pos2, const int32_t* sup, int32_t n_sup,
+                            int32_t bias, int32_t gt_round, const csv_geno* gl_table) {
+    return tra_call_gt_rules(TraCountCoverage{}, A, chr1, pos1, chr2, pos2, sup, n_sup, bias, gt_round, gl_table);
+}
+// One TRA candidate of csv_cluster (chr2 = aux >> 2); sup: its names slice.
+CSV_HD void tra_call_gt(const AlnView& A, const csv_cand& c, const int32_t* sup, int32_t bias, int32_t gt_round, const csv_geno* gl_table,
+                        csv_geno* g) {
+    *g = tra_call_gt(A, c.chrom, c.pos, c.aux >> 2, c.pos2, sup, c.names_cnt, bias, gt_round, gl_table);
 }
 
 // ------------------------------------------------------------------------------------------

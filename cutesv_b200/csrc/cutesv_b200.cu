@@ -181,10 +181,12 @@ struct LbPool {
     int next = 0, cap = 0;
 };
 
-// scratch of csv_overlap_cover / csv_call_gt (genotype_api.inl): separate from everything csv_cluster uses
+// scratch of csv_overlap_cover / csv_call_gt / csv_tra_call_gt (genotype_api.inl): separate from everything csv_cluster uses.
+// csv_tra_call_gt keeps a host alignment table in r_* and its contig index in a_off / a_span.
 struct GcWork {
     DBuf win, bin_base, bin_start, bin_fill, bin_list, iter, prim, cov_off, ovl_off, cov_fill, ovl_fill, cov_u, ovl_u, lb, words;
     DBuf r_chrom, r_start, r_end, r_id, r_prim, cov_raw, ovl_raw, cov_ded, ovl_ded, cov_flag, ovl_flag, sup_off, sup, geno;
+    DBuf tra_q, a_off, a_span;
     uint32_t n_cov = 0, n_ovl = 0;   // raw ids of the last call
 };
 
@@ -843,25 +845,26 @@ extern "C" int csv_upload_reads_grouped_device(csv_ctx* c, const csv_reads_cols*
     return upload_reads_impl(c, d, contig_off, UpSrc{true, (cudaStream_t)stream});
 }
 
-// Contig index + sortedness check of the n rows in c->a_* (BAM order is a precondition of the early-exit scan); one
-// synchronisation.  A failure leaves no table.
-static int aln_index(csv_ctx* c, int64_t n) {
+// Contig index (off, span: n_contigs + 2 entries) + sortedness check of the n rows of an alignment table (BAM order is a
+// precondition of the early-exit scan); one synchronisation.  A failure of the ctx's own table (c->a_*) leaves no table.
+static int aln_index(csv_ctx* c, int64_t n, const DBuf& chrom, const DBuf& start, const DBuf& end, DBuf& off, DBuf& span) {
     CU(c->aln_flag.ensure(64));
     uint32_t* flag = c->aln_flag.as<uint32_t>();
     CU(cudaMemsetAsync(flag, 0, 4, c->stream));
-    CU(cudaMemsetAsync(c->a_span.p, 0, ((size_t)c->n_contigs + 2) * 4, c->stream));
-    LAUNCH(c, c->stream, k_aln_index, grid_for(c, n, 256), 256, 0, c->a_chrom.as<int32_t>(), c->a_start.as<int32_t>(), c->a_end.as<int32_t>(), n,
-           c->n_contigs, c->a_span.as<int32_t>(), flag);
-    LAUNCH(c, c->stream, k_aln_off, grid_for(c, (int64_t)c->n_contigs + 1, 256), 256, 0, c->a_chrom.as<int32_t>(), n, c->n_contigs, c->a_off.as<uint32_t>());
+    CU(cudaMemsetAsync(span.p, 0, ((size_t)c->n_contigs + 2) * 4, c->stream));
+    LAUNCH(c, c->stream, k_aln_index, grid_for(c, n, 256), 256, 0, chrom.as<int32_t>(), start.as<int32_t>(), end.as<int32_t>(), n,
+           c->n_contigs, span.as<int32_t>(), flag);
+    LAUNCH(c, c->stream, k_aln_off, grid_for(c, (int64_t)c->n_contigs + 1, 256), 256, 0, chrom.as<int32_t>(), n, c->n_contigs, off.as<uint32_t>());
     uint32_t hflag = 0;
     CU(cudaMemcpyAsync(&hflag, flag, 4, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     if (hflag) {
-        c->n_aln = 0;
+        if (&chrom == &c->a_chrom) c->n_aln = 0;
         return set_err(CSV_E_INPUT, "alignment table: %s", (hflag & ST_UNSORTED) ? "not coordinate-sorted (BAM order required)" : "contig id out of range");
     }
     return CSV_OK;
 }
+static int aln_index(csv_ctx* c, int64_t n) { return aln_index(c, n, c->a_chrom, c->a_start, c->a_end, c->a_off, c->a_span); }
 
 // The alignment table is copied on the ctx stream and its order is checked before the call returns (one synchronisation, for host
 // and device columns alike), so a device source's buffers are free again on return.

@@ -57,7 +57,7 @@ inline std::vector<csv_geno> build_gl_table() {
         for (int c1 = 0; c1 <= 100; c1++) {
             csv_geno g;
             g.dr = c0; g.dv = c1; g.gt = -1; g.pl[0] = g.pl[1] = g.pl[2] = 0; g.gq = 0; g.status = 1; g.qual = 0.0;
-            if (c0 + c1 <= 100 && c0 + c1 > 0) host_cal_gl_core(c0, c1, &g);
+            if (c0 + c1 <= 100) host_cal_gl_core(c0, c1, &g);   // (0, 0): call_gt of resolveTRA with no supporting reads
             t[c0 * 101 + c1] = g;
         }
     csv_geno s;

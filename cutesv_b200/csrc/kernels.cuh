@@ -1535,6 +1535,17 @@ __device__ __forceinline__ int tra_count_coverage_warp(const AlnView& A, int32_t
     }
     return 0;
 }
+struct TraCountCoverageWarp {
+    __device__ __forceinline__ int operator()(const AlnView& A, int32_t chr, int64_t s, int64_t e, const int32_t* sup, int n_sup, int32_t up_bound,
+                                              int32_t itround, int32_t* nset, int32_t* dr, int64_t xs, int64_t xe) const {
+        return tra_count_coverage_warp(A, chr, s, e, sup, n_sup, up_bound, itround, nset, dr, xs, xe);
+    }
+};
+// call_gt of one breakpoint pair by one warp (core.h tra_call_gt_rules); every lane returns the same csv_geno
+__device__ __forceinline__ csv_geno tra_call_gt_warp(const AlnView& A, int32_t chr1, int64_t pos1, int32_t chr2, int64_t pos2, const int32_t* sup,
+                                                     int32_t n_sup, int32_t bias, int32_t gt_round, const csv_geno* gl_table) {
+    return tra_call_gt_rules(TraCountCoverageWarp{}, A, chr1, pos1, chr2, pos2, sup, n_sup, bias, gt_round, gl_table);
+}
 // one warp per TRA candidate; the candidates are ordered by SV type, TRA last, so warp w takes candidate n-1-w
 __global__ void __launch_bounds__(128) k_tra_genotype(GenoJob G, AlnView A, int32_t bias, int32_t gt_round) {
     const uint32_t n = min(G.ctr->n_cand, G.cap_cand);
@@ -1544,31 +1555,24 @@ __global__ void __launch_bounds__(128) k_tra_genotype(GenoJob G, AlnView A, int3
         const uint32_t i = n - 1 - w;
         const csv_cand c = G.cand[i];
         if (c.svtype != CSV_TRA) break;   // uniform across the warp
-        const int32_t* sup = G.names + c.names_off;
-        const int32_t chr1 = c.chrom, chr2 = c.aux >> 2, n_sup = c.names_cnt;
-        const int32_t up = threshold_ref_count(n_sup);
-        int32_t nset = 0, dr = 0;
-        int64_t s = (int64_t)c.pos - bias; if (s < 0) s = 0;
-        int64_t e = (int64_t)c.pos + bias; if (e > A.contig_len[chr1]) e = A.contig_len[chr1];
-        const int st = tra_count_coverage_warp(A, chr1, s, e, sup, n_sup, up, gt_round, &nset, &dr, 1, 0);
-        const int64_t s1 = s, e1 = e;
-        csv_geno g;
-        if (st == -1) {  // DR '.', GT './.' (resolveTRA.py:277-282)
-            g.dr = -1; g.dv = n_sup; g.gt = -1; g.pl[0] = g.pl[1] = g.pl[2] = 0; g.gq = 0; g.status = 2; g.qual = 0.0;
-        } else {
-            if (st == 0) {
-                s = (int64_t)c.pos2 - bias; if (s < 0) s = 0;
-                e = (int64_t)c.pos2 + bias; if (e > A.contig_len[chr2]) e = A.contig_len[chr2];
-                if (chr2 == chr1) tra_count_coverage_warp(A, chr2, s, e, sup, n_sup, up, gt_round, &nset, &dr, s1, e1);
-                else tra_count_coverage_warp(A, chr2, s, e, sup, n_sup, up, gt_round, &nset, &dr, 1, 0);
-            }
-            g = G.gl_table[gl_index(dr, n_sup)];
-            g.dr = dr; g.dv = n_sup;
-        }
+        const csv_geno g = tra_call_gt_warp(A, c.chrom, c.pos, c.aux >> 2, c.pos2, G.names + c.names_off, c.names_cnt, bias, gt_round, G.gl_table);
         if (lane == 0) {
             G.geno[i] = g;
             G.cand[i].flags = c.flags & ~CSV_F_GT_HOST;
         }
+    }
+}
+
+// csv_tra_call_gt: one warp per caller-given breakpoint pair; query i's supporting ids are sup[sup_off[i], sup_off[i + 1]), ascending
+__global__ void __launch_bounds__(128) k_tra_call_gt(const csv_tra_query* __restrict__ q, uint32_t n, const int64_t* __restrict__ sup_off,
+                                                     const int32_t* __restrict__ sup, AlnView A, int32_t bias, int32_t gt_round,
+                                                     const csv_geno* __restrict__ gl_table, csv_geno* __restrict__ out) {
+    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, n_warps = (gridDim.x * blockDim.x) >> 5;
+    for (uint32_t i = warp; i < n; i += n_warps) {
+        const csv_tra_query x = q[i];
+        const int64_t so = sup_off[i];
+        const csv_geno g = tra_call_gt_warp(A, x.chr1, x.pos1, x.chr2, x.pos2, sup + so, (int32_t)(sup_off[i + 1] - so), bias, gt_round, gl_table);
+        if ((threadIdx.x & 31) == 0) out[i] = g;
     }
 }
 

@@ -5,7 +5,9 @@
 - assign_gt (:161-173): DR from the given sets on the host, cal_GL batched through csv_cal_gl.
 - cal_CIPOS (:58-60) and threshold_ref_count (:62-70): host arithmetic, the same expressions.
 
-count_coverage (:72-93) needs a BAM handle; TRA genotyping runs on the device inside csv_cluster instead.
+count_coverage (:72-93) takes a pysam handle and fills the caller's name set, so it has no drop-in of its own; its one
+caller, resolveTRA's call_gt, has one (cuteSV_resolveTRA.call_gt, csv_tra_call_gt), which scans a table of the records
+decoded around its windows.
 call_gt of resolveINDEL / resolveDUP / resolveINV uses call_gt_genos below (csv_call_gt)."""
 import numpy as np
 

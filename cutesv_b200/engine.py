@@ -282,6 +282,25 @@ class Engine(object):
         del keep
         return out[:n]
 
+    def tra_call_gt(self, queries, support_off, support_ids, bias, gt_round, aln=None):
+        """call_gt of resolveTRA.py:260-309 on the device for caller-given breakpoint pairs (_abi.TRA_QUERY_DTYPE; contig ids of the
+        set_contigs table, whose lengths clamp the windows).  Query i's supporting read ids are support_ids[support_off[i]:support_off[i+1]]
+        (DV = their count).  aln: host all-alignments columns in BAM order (dict like the reads table), or None for the table
+        installed by upload_alignments / rank_names.  Returns a GENO_DTYPE array: cal_GL(DR, DV) with dr / dv, or status 2 with
+        dr = gt = -1 where the first window's scan returns -1."""
+        q = np.ascontiguousarray(queries, dtype=_abi.TRA_QUERY_DTYPE)
+        so = np.ascontiguousarray(support_off, dtype=np.int64)
+        si = np.ascontiguousarray(support_ids, dtype=np.int32)
+        n = len(q)
+        assert len(so) == n + 1
+        r, keep = _abi.make_reads_cols(aln) if aln is not None else (None, ())
+        out = np.zeros(max(n, 1), dtype=_abi.GENO_DTYPE)
+        _lib.check(self.L.csv_tra_call_gt(self.h, q.ctypes.data_as(C.c_void_p), C.c_int64(n), C.byref(r) if r is not None else None,
+                                          C.c_int32(bias), C.c_int32(gt_round), so.ctypes.data_as(C.POINTER(C.c_int64)), _abi.ptr(si),
+                                          out.ctypes.data_as(C.c_void_p)))
+        del keep
+        return out[:n]
+
     def sort_sigs(self, svtype):
         """Sort + adjacent de-duplication of process_process_sigs_type (cuteSV:750-857, 958-969) over the device-resident
         columns of one type (name or id) or of the reads table ("reads").  Returns dict(order, contig_off, ins_tie): the input

@@ -285,6 +285,30 @@ int csv_overlap_cover(csv_ctx* ctx, const csv_window* windows, int64_t n_windows
 int csv_call_gt(csv_ctx* ctx, const csv_window* windows, int64_t n_cand, int32_t windows_per_cand, const csv_reads_cols* reads,
                 const int64_t* support_off, const int32_t* support_ids, csv_geno* out);
 
+/* ---- standalone TRA genotyper: the call_gt of resolveTRA.py:260-309 (count_coverage, cuteSV_genotype.py:72-93) for
+ * caller-given breakpoint pairs over an all-alignments table in BAM order ----
+ *
+ * Query i scans the window [max(pos1 - bias, 0), min(pos1 + bias, len(chr1))] of chr1 and, when that scan ends without
+ * an early return, the same window around pos2 on chr2; contig lengths come from csv_set_contigs.  A record is fetched by
+ * a window [s, e] iff start < e and end > s.  support_off (n + 1) / support_ids: every query's supporting read ids in any
+ * order, duplicates allowed; DV = the segment's length, membership is by id.
+ *   - the first scan returns -1 (more than 20% primary records at gt_round): out[i] = {dr -1, dv, gt -1, status 2};
+ *   - otherwise out[i] = cal_GL(DR, DV) with dr / dv filled (the second scan's status is not used, as in the reference).
+ * aln: host columns (chrom, start, end, read_id, is_primary = flag in (0, 16)), copied into the call's own scratch; NULL
+ * uses the table installed by csv_upload_alignments* / csv_rank_names (CSV_E_STATE when there is none).  Precondition, as
+ * for that table: one primary record per read name.
+ * Errors, all found before any launch except the table's order (CSV_E_INPUT), and none changing the ctx:
+ *   CSV_E_INVALID  a null pointer, n outside [0, 2^29), bias < 0, support_off not starting at 0 or decreasing;
+ *   CSV_E_INPUT    a contig id outside the contig table or a clamped window with start > end (pysam's fetch raises
+ *                  ValueError), naming the query; a table not in BAM order or with a contig id out of range.
+ * Blocks until out is on the host.  Leaves csv_cluster's inputs, results, alignment table and captured graphs alone. */
+typedef struct csv_tra_query {
+    int32_t chr1, chr2;   /* contig ids of the two breakpoints */
+    int64_t pos1, pos2;
+} csv_tra_query;
+int csv_tra_call_gt(csv_ctx* ctx, const csv_tra_query* q, int64_t n, const csv_reads_cols* aln, int32_t bias, int32_t gt_round,
+                    const int64_t* support_off, const int32_t* support_ids, csv_geno* out);
+
 /* ---- standalone signature rebuild: the sort + remove_duplicates_sorted of process_process_sigs_type (cuteSV:750-857,
  * 958-969) over the device-resident columns of ONE type (svtype CSV_DEL..CSV_TRA) or of the reads table
  * (svtype CSV_SORT_READS), i.e. whatever csv_upload_sigs / csv_upload_reads (grouped or not) or csv_extract* put there ----
