@@ -83,14 +83,159 @@ struct DBuf {
         }
         return cudaSuccess;
     }
+    // capacity for `bytes`, keeping the first keep_bytes of the present contents (append mode: copied on s, which is then
+    // synchronised)
+    cudaError_t grow(size_t bytes, size_t keep_bytes, cudaStream_t s) {
+        if (bytes <= cap) return cudaSuccess;
+        if (keep_bytes == 0 || !p) return ensure(bytes);
+        DBuf nb;
+        cudaError_t e = nb.ensure(bytes + bytes / 2);   // geometric growth: a run appends many packets
+        if (e == cudaSuccess) e = cudaMemcpyAsync(nb.p, p, keep_bytes, cudaMemcpyDeviceToDevice, s);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+        if (e == cudaSuccess) *this = std::move(nb);   // frees the old buffer
+        return e;
+    }
+    // D2H of bytes [off, off + bytes), when the caller asked for them (dst not null)
+    cudaError_t fetch(void* dst, size_t off, size_t bytes, cudaStream_t s) const {
+        return dst && bytes ? cudaMemcpyAsync(dst, (const char*)p + off, bytes, cudaMemcpyDeviceToHost, s) : cudaSuccess;
+    }
     void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
     template <class T> T* as() const { return (T*)p; }
 };
 
-struct SigBuf {
+// ------------------------------------------------------------------------------------------
+// input tables: the only place that knows their columns; callers size, grow, fill, check and fetch whole tables
+// ------------------------------------------------------------------------------------------
+static int check_dev_col(const csv_ctx* c, const void* p, const char* name);
+
+// the pending and installed alignment rows of a scanned accumulation (k_scan_aln, k_scan_aln_gather)
+struct AlnCols {
+    int32_t *chrom, *start, *end, *id;
+    uint8_t* prim;
+};
+// csv_sort_sigs' columns of one type (sigsort_api.inl)
+struct SsCols {
+    const int32_t *chrom, *a, *b, *rid, *c;
+    int type;
+};
+
+// The signatures of one SV type: contig, a, b, read id and (INS / INV / TRA) c, 4 B per row each
+struct SigTable {
     int64_t n = 0;
     bool has_c = false;
     DBuf chrom, a, b, rid, c;
+    // capacity for `rows` rows of every column but c, which copy_in sizes when the source carries it
+    int size(int64_t rows) {
+        const size_t bytes = (size_t)rows * 4;
+        for (DBuf* col : {&chrom, &a, &b, &rid}) CU(col->ensure(bytes));
+        return CSV_OK;
+    }
+    // capacity for `rows` rows of all five columns, keeping the first keep_rows (append mode)
+    int grow(int64_t rows, int64_t keep_rows, cudaStream_t s) {
+        for (DBuf* col : {&chrom, &a, &b, &rid, &c}) CU(col->grow((size_t)rows * 4, (size_t)keep_rows * 4, s));
+        return CSV_OK;
+    }
+    // the caller's h.n rows; without chrom for a grouped upload (k_expand_contigs writes it)
+    int copy_in(const csv_sig_cols& h, bool with_chrom, cudaMemcpyKind kind, cudaStream_t s) {
+        const size_t bytes = (size_t)h.n * 4;
+        if (with_chrom) CU(cudaMemcpyAsync(chrom.p, h.chrom, bytes, kind, s));
+        CU(cudaMemcpyAsync(a.p, h.a, bytes, kind, s));
+        CU(cudaMemcpyAsync(b.p, h.b, bytes, kind, s));
+        CU(cudaMemcpyAsync(rid.p, h.read_id, bytes, kind, s));
+        if (h.c) { CU(c.ensure(bytes)); CU(cudaMemcpyAsync(c.p, h.c, bytes, kind, s)); }
+        return CSV_OK;
+    }
+    // device uploads: every non-null column of h is device memory of the ctx's device
+    static int check_dev(const csv_ctx* ctx, const csv_sig_cols& h, bool with_chrom) {
+        const void* col[5] = {with_chrom ? h.chrom : nullptr, h.a, h.b, h.read_id, h.c};
+        static const char* const nm[5] = {"chrom", "a", "b", "read_id", "c"};
+        for (int k = 0; k < 5; k++) { int rc = check_dev_col(ctx, col[k], nm[k]); if (rc) return rc; }
+        return CSV_OK;
+    }
+    // rows [first, first + count) into the host columns that are not null (c only when the table has it); not synchronised
+    int fetch(int64_t first, int64_t count, int32_t* h_chrom, int32_t* h_a, int32_t* h_b, int32_t* h_rid, int32_t* h_c, cudaStream_t s) const {
+        const size_t bytes = (size_t)count * 4, o = (size_t)first * 4;
+        CU(chrom.fetch(h_chrom, o, bytes, s)); CU(a.fetch(h_a, o, bytes, s)); CU(b.fetch(h_b, o, bytes, s)); CU(rid.fetch(h_rid, o, bytes, s));
+        if (has_c) CU(c.fetch(h_c, o, bytes, s));
+        return CSV_OK;
+    }
+    // chrom, a, b, rid, c: the order of ExtractOut::col[t], TieCols::col and k_swap_rows
+    void cols(int32_t* col[5]) const {
+        col[0] = chrom.as<int32_t>(); col[1] = a.as<int32_t>(); col[2] = b.as<int32_t>(); col[3] = rid.as<int32_t>(); col[4] = c.as<int32_t>();
+    }
+    SsCols sort_cols(int type) const {
+        return SsCols{chrom.as<int32_t>(), a.as<int32_t>(), b.as<int32_t>(), rid.as<int32_t>(), has_c ? c.as<int32_t>() : nullptr, type};
+    }
+};
+
+// Rows shaped like the reads table: contig, start, end, read id (4 B each) and is_primary (1 B unless sized wider)
+struct RowTable {
+    int64_t n = 0;
+    DBuf chrom, start, end, rid, prim;
+    // capacity for `rows` rows; prim_size: bytes per is_primary entry
+    int size(int64_t rows, size_t prim_size = 1) {
+        const size_t bytes = (size_t)rows * 4;
+        for (DBuf* col : {&chrom, &start, &end, &rid}) CU(col->ensure(bytes));
+        CU(prim.ensure((size_t)rows * prim_size));
+        return CSV_OK;
+    }
+    // capacity for `rows` rows, keeping the first keep_rows (append mode)
+    int grow(int64_t rows, int64_t keep_rows, cudaStream_t s) {
+        for (DBuf* col : {&chrom, &start, &end, &rid}) CU(col->grow((size_t)rows * 4, (size_t)keep_rows * 4, s));
+        CU(prim.grow((size_t)rows, (size_t)keep_rows, s));
+        return CSV_OK;
+    }
+    // h has every column the copy needs (a grouped upload has no chrom)
+    static bool has_cols(const csv_reads_cols& h, bool with_chrom) {
+        return (!with_chrom || h.chrom) && h.start && h.end && h.read_id && h.is_primary;
+    }
+    // the caller's h.n rows; without chrom for a grouped upload (k_expand_contigs writes it)
+    int copy_in(const csv_reads_cols& h, bool with_chrom, cudaMemcpyKind kind, cudaStream_t s) {
+        if (h.n == 0) return CSV_OK;
+        const size_t bytes = (size_t)h.n * 4;
+        if (with_chrom) CU(cudaMemcpyAsync(chrom.p, h.chrom, bytes, kind, s));
+        CU(cudaMemcpyAsync(start.p, h.start, bytes, kind, s));
+        CU(cudaMemcpyAsync(end.p, h.end, bytes, kind, s));
+        CU(cudaMemcpyAsync(rid.p, h.read_id, bytes, kind, s));
+        CU(cudaMemcpyAsync(prim.p, h.is_primary, (size_t)h.n, kind, s));
+        return CSV_OK;
+    }
+    // device uploads: every non-null column of h is device memory of the ctx's device
+    static int check_dev(const csv_ctx* ctx, const csv_reads_cols& h, bool with_chrom) {
+        const void* col[5] = {with_chrom ? h.chrom : nullptr, h.start, h.end, h.read_id, h.is_primary};
+        static const char* const nm[5] = {"chrom", "start", "end", "read_id", "is_primary"};
+        for (int k = 0; k < 5; k++) { int rc = check_dev_col(ctx, col[k], nm[k]); if (rc) return rc; }
+        return CSV_OK;
+    }
+    // rows [first, first + count) into the host columns that are not null; not synchronised
+    int fetch(int64_t first, int64_t count, int32_t* h_chrom, int32_t* h_start, int32_t* h_end, int32_t* h_rid, uint8_t* h_prim,
+              cudaStream_t s) const {
+        const size_t bytes = (size_t)count * 4, o = (size_t)first * 4;
+        CU(chrom.fetch(h_chrom, o, bytes, s)); CU(start.fetch(h_start, o, bytes, s)); CU(end.fetch(h_end, o, bytes, s));
+        CU(rid.fetch(h_rid, o, bytes, s)); CU(prim.fetch(h_prim, (size_t)first, (size_t)count, s));
+        return CSV_OK;
+    }
+    AlnCols cols() const { return AlnCols{chrom.as<int32_t>(), start.as<int32_t>(), end.as<int32_t>(), rid.as<int32_t>(), prim.as<uint8_t>()}; }
+    GcReads gc_reads() const { return GcReads{chrom.as<int32_t>(), start.as<int32_t>(), end.as<int32_t>(), rid.as<int32_t>(), prim.as<uint8_t>(), n}; }
+    // k_extract's reads-row outputs
+    void extract_out(ExtractOut& O) const {
+        O.rr_chrom = chrom.as<int32_t>(); O.rr_start = start.as<int32_t>(); O.rr_end = end.as<int32_t>(); O.rr_id = rid.as<int32_t>();
+        O.rr_prim = prim.as<uint8_t>();
+    }
+};
+
+// An alignment table (BAM order) and its contig index of aln_index: first row (off) and longest row (span) per contig
+struct AlnTable : RowTable {
+    DBuf off, span;
+    int size_index(int32_t n_contigs) {
+        const size_t bytes = ((size_t)n_contigs + 2) * 4;
+        CU(off.ensure(bytes)); CU(span.ensure(bytes));
+        return CSV_OK;
+    }
+    AlnView view(const int64_t* contig_len) const {
+        return AlnView{chrom.as<int32_t>(), start.as<int32_t>(), end.as<int32_t>(), rid.as<int32_t>(), prim.as<uint8_t>(), off.as<uint32_t>(),
+                       span.as<int32_t>(), contig_len};
+    }
 };
 
 struct SmallWork {  // DUP / INV / TRA
@@ -103,6 +248,15 @@ struct SmallWork {  // DUP / INV / TRA
 enum class PacketKind { PLAIN, NAMED, SCANNED, SCANNED_ALN };
 static inline bool kind_named(PacketKind k) { return k != PacketKind::PLAIN; }
 static inline bool kind_scanned(PacketKind k) { return k == PacketKind::SCANNED || k == PacketKind::SCANNED_ALN; }
+
+// Upload state of one input slot: the signatures of an SV type, or the reads table
+struct UploadSlot {
+    cudaEvent_t ev = nullptr;   // end of the slot's last upload on the copy stream
+    bool pending = false;       // ... not yet waited for
+    bool device = false;        // the pending upload copies device memory
+    bool checked = false;       // the slot's offsets were checked on the device
+    DBuf goff;                  // contig row offsets of a grouped upload
+};
 
 // Pinned staging of the extraction stage's small copies, one field per use
 struct ExStaging {
@@ -138,11 +292,11 @@ struct ExtractState {
     bool ranked = false;             // csv_rank_names has turned the provisional ids into ranks
     int64_t name_nbytes = 0, n_names = 0;
     // scanned accumulation (csv_scan_append_named_device, scan_api.inl): every decoded record of each packet.  scan_flag is the
-    // packet's flag column with 256 on every record the reference would not extract; p_* the pending alignment table (BAM
-    // order, provisional ids) that csv_rank_names installs; rg_* the region table of csv_set_scan_regions.
-    DBuf scan_flag, scan_excl, p_chrom, p_start, p_end, p_id, p_prim;
+    // packet's flag column with 256 on every record the reference would not extract; pending the alignment rows (BAM order,
+    // provisional ids) that csv_rank_names installs; rg_* the region table of csv_set_scan_regions.
+    DBuf scan_flag, scan_excl;
+    RowTable pending;
     DBuf rg_win_off, rg_win_start, rg_reg_off, rg_reg;
-    int64_t n_pending = 0;
     int32_t rg_n_contigs = 0;        // 0: no region table
     double per_record[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // largest yield of a packet so far: signatures per type [0..4], pieces [5] per alignment record
 };
@@ -182,11 +336,12 @@ struct LbPool {
 };
 
 // scratch of csv_overlap_cover / csv_call_gt / csv_tra_call_gt (genotype_api.inl): separate from everything csv_cluster uses.
-// csv_tra_call_gt keeps a host alignment table in r_* and its contig index in a_off / a_span.
+// The host tables of the calls are copied into aln: the drop-ins' reads table (rows only), csv_tra_call_gt's alignment table.
 struct GcWork {
     DBuf win, bin_base, bin_start, bin_fill, bin_list, iter, prim, cov_off, ovl_off, cov_fill, ovl_fill, cov_u, ovl_u, lb, words;
-    DBuf r_chrom, r_start, r_end, r_id, r_prim, cov_raw, ovl_raw, cov_ded, ovl_ded, cov_flag, ovl_flag, sup_off, sup, geno;
-    DBuf tra_q, a_off, a_span;
+    DBuf cov_raw, ovl_raw, cov_ded, ovl_ded, cov_flag, ovl_flag, sup_off, sup, geno;
+    DBuf tra_q;
+    AlnTable aln;
     uint32_t n_cov = 0, n_ovl = 0;   // raw ids of the last call
 };
 
@@ -202,10 +357,7 @@ struct csv_ctx {
     // uploads run on their own stream so that the H2D copy of the next SV type / the reads table
     // overlaps the kernels of the previous type (e2e is PCIe-bound)
     cudaStream_t copy_stream = nullptr;
-    cudaEvent_t ev_up[CSV_NTYPES + 1] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};  // last: reads table
-    bool up_pending[CSV_NTYPES + 1] = {false, false, false, false, false, false};
-    bool up_device[CSV_NTYPES + 1] = {false, false, false, false, false, false};    // the pending upload copies device memory
-    bool up_checked[CSV_NTYPES + 1] = {false, false, false, false, false, false};   // the slot's offsets were checked on the device
+    UploadSlot up[CSV_NTYPES + 1];   // last: reads table
     DBuf up_status;                  // one word per slot: k_check_contig_off's result, folded into the next csv_cluster's status
     cudaEvent_t ev_prod = nullptr;   // device uploads: end of the caller's work on its producer stream
     cudaEvent_t ev_done = nullptr;   // end of the last csv_cluster on the compute stream
@@ -221,11 +373,9 @@ struct csv_ctx {
     std::vector<uint8_t> owned;     // csv_set_shard: contigs this ctx works on (empty = all)
     DBuf d_off, d_len, d_len_eff;   // d_len_eff: -1 for contigs outside the shard (input validation)
     // inputs
-    SigBuf sig[CSV_NTYPES];
-    int64_t n_reads = 0;
-    DBuf r_chrom, r_start, r_end, r_id, r_prim;
-    int64_t n_aln = 0;
-    DBuf a_chrom, a_start, a_end, a_id, a_prim, a_off, a_span;
+    SigTable sig[CSV_NTYPES];
+    RowTable reads;
+    AlnTable aln;
     DBuf tickets, scan_carry, emit_cursor;
     DBuf d_epoch;                    // look-back generation base, bumped by the first kernel of every csv_cluster
     LbPool lb;                       // csv_cluster's look-back tickets, shared by its lanes (ordinals stay unique per call)
@@ -235,7 +385,6 @@ struct csv_ctx {
     bool records_enabled = true;
     bool small_path_enabled = true;
     int64_t pair_cap_override = 0;
-    DBuf d_goff[CSV_NTYPES + 1];   // contig row offsets of grouped uploads (last: reads table)
     Lane lanes[N_LANES];           // lanes[0].stream is `stream`
     cudaEvent_t ev_fork = nullptr;
     cudaStream_t side_stream[2] = {nullptr, nullptr};   // DEL / INS: the general cluster kernels beside the register kernel
@@ -494,7 +643,7 @@ extern "C" int csv_create(int device, void* stream, csv_ctx** out) {
     c->lanes[0].stream = c->stream;
     {
         cudaError_t e4 = cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking);
-        for (int i = 0; i <= CSV_NTYPES && e4 == cudaSuccess; i++) e4 = cudaEventCreateWithFlags(&c->ev_up[i], cudaEventDisableTiming);
+        for (UploadSlot& u : c->up) if (e4 == cudaSuccess) e4 = cudaEventCreateWithFlags(&u.ev, cudaEventDisableTiming);
         if (e4 == cudaSuccess) e4 = cudaEventCreateWithFlags(&c->ev_done, cudaEventDisableTiming);
         if (e4 == cudaSuccess) e4 = cudaEventCreateWithFlags(&c->ev_prod, cudaEventDisableTiming);
         if (e4 == cudaSuccess) e4 = cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming);
@@ -573,7 +722,7 @@ extern "C" int csv_destroy(csv_ctx* c) {
     for (cudaEvent_t e : c->ev_pool) cudaEventDestroy(e);
     if (c->h_counters) cudaFreeHost(c->h_counters);
     if (c->copy_stream) { cudaStreamSynchronize(c->copy_stream); cudaStreamDestroy(c->copy_stream); }
-    for (int i = 0; i <= CSV_NTYPES; i++) if (c->ev_up[i]) cudaEventDestroy(c->ev_up[i]);
+    for (UploadSlot& u : c->up) if (u.ev) cudaEventDestroy(u.ev);
     if (c->ev_done) cudaEventDestroy(c->ev_done);
     if (c->ev_prod) cudaEventDestroy(c->ev_prod);
     if (c->own_stream) cudaStreamDestroy(c->stream);
@@ -710,16 +859,18 @@ static int upload_begin(csv_ctx* c, const UpSrc& src) {
     return CSV_OK;
 }
 static int upload_end(csv_ctx* c, int slot, const UpSrc& src) {
-    CU(cudaEventRecord(c->ev_up[slot], c->copy_stream));
-    if (src.device) CU(cudaStreamWaitEvent(src.producer, c->ev_up[slot], 0));
-    c->up_pending[slot] = true;
-    c->up_device[slot] = src.device;
+    UploadSlot& u = c->up[slot];
+    CU(cudaEventRecord(u.ev, c->copy_stream));
+    if (src.device) CU(cudaStreamWaitEvent(src.producer, u.ev, 0));
+    u.pending = true;
+    u.device = src.device;
     return CSV_OK;
 }
 static int wait_upload(csv_ctx* c, cudaStream_t s, int slot) {
-    if (c->up_pending[slot]) {
-        CU(cudaStreamWaitEvent(s, c->ev_up[slot], 0));
-        c->up_pending[slot] = false;
+    UploadSlot& u = c->up[slot];
+    if (u.pending) {
+        CU(cudaStreamWaitEvent(s, u.ev, 0));
+        u.pending = false;
     }
     return CSV_OK;
 }
@@ -734,17 +885,18 @@ static int stage_group_offsets(csv_ctx* c, int slot, const int64_t* off, int64_t
         for (int k = 0; k < c->n_contigs; k++)
             if (off[k + 1] < off[k]) return set_err(CSV_E_INVALID, "contig_off must be non-decreasing");
     }
-    CU(c->d_goff[slot].ensure(((size_t)c->n_contigs + 1) * 8));
-    CU(cudaMemcpyAsync(c->d_goff[slot].p, off, ((size_t)c->n_contigs + 1) * 8, src.kind(), c->copy_stream));
+    UploadSlot& u = c->up[slot];
+    CU(u.goff.ensure(((size_t)c->n_contigs + 1) * 8));
+    CU(cudaMemcpyAsync(u.goff.p, off, ((size_t)c->n_contigs + 1) * 8, src.kind(), c->copy_stream));
     uint32_t* bad = nullptr;
     if (src.device) {
         bad = c->up_status.as<uint32_t>() + slot;
         CU(cudaMemsetAsync(bad, 0, 4, c->copy_stream));
-        k_check_contig_off<<<grid_for(c, (int64_t)c->n_contigs + 1, 256), 256, 0, c->copy_stream>>>(c->d_goff[slot].as<int64_t>(), c->n_contigs, n, bad);
+        k_check_contig_off<<<grid_for(c, (int64_t)c->n_contigs + 1, 256), 256, 0, c->copy_stream>>>(u.goff.as<int64_t>(), c->n_contigs, n, bad);
         c->launches++;
-        c->up_checked[slot] = true;
+        u.checked = true;
     }
-    k_expand_contigs<<<grid_for(c, n, 256 * 4), 256, 0, c->copy_stream>>>(c->d_goff[slot].as<int64_t>(), c->n_contigs, n, chrom_dev, bad);
+    k_expand_contigs<<<grid_for(c, n, 256 * 4), 256, 0, c->copy_stream>>>(u.goff.as<int64_t>(), c->n_contigs, n, chrom_dev, bad);
     c->launches++;
     return CSV_OK;
 }
@@ -756,15 +908,15 @@ static void inputs_replaced(csv_ctx* c, int slot) {
     c->ex.rec_valid = false;
     c->ex.seq_valid = false;
     c->ex.kind = PacketKind::PLAIN; c->ex.ranked = false;
-    c->ex.n_pending = 0;
-    c->up_checked[slot] = false;
+    c->ex.pending.n = 0;
+    c->up[slot].checked = false;
 }
 
 static int upload_sigs_impl(csv_ctx* c, int t, const csv_sig_cols* h, const int64_t* contig_off, const UpSrc& src) {
     if (!c || t < 0 || t >= CSV_NTYPES || !h) return set_err(CSV_E_INVALID, "bad argument");
     if (h->n < 0 || h->n >= (1ll << 30)) return set_err(CSV_E_INVALID, "signature count %lld out of range", (long long)h->n);
     CU(cudaSetDevice(c->device));
-    SigBuf& s = c->sig[t];
+    SigTable& s = c->sig[t];
     s.n = h->n;
     s.has_c = h->c != nullptr;
     inputs_replaced(c, t);
@@ -772,22 +924,10 @@ static int upload_sigs_impl(csv_ctx* c, int t, const csv_sig_cols* h, const int6
     if ((!contig_off && !h->chrom) || !h->a || !h->b || !h->read_id) return set_err(CSV_E_INVALID, "null column");
     if ((t == CSV_INS || t == CSV_INV || t == CSV_TRA) && !h->c) return set_err(CSV_E_INVALID, "column c is required for INS/INV/TRA");
     int rc;
-    if (src.device) {
-        const void* col[6] = {contig_off ? nullptr : h->chrom, h->a, h->b, h->read_id, h->c, contig_off};
-        static const char* const nm[6] = {"chrom", "a", "b", "read_id", "c", "contig_off"};
-        for (int k = 0; k < 6; k++) if ((rc = check_dev_col(c, col[k], nm[k]))) return rc;
-    }
-    const size_t bytes = (size_t)h->n * 4;
-    const cudaMemcpyKind kind = src.kind();
-    rc = upload_begin(c, src);
-    if (rc) return rc;
-    CU(s.chrom.ensure(bytes)); CU(s.a.ensure(bytes)); CU(s.b.ensure(bytes)); CU(s.rid.ensure(bytes));
-    if (contig_off) { rc = stage_group_offsets(c, t, contig_off, h->n, s.chrom.as<int32_t>(), src); if (rc) return rc; }
-    else CU(cudaMemcpyAsync(s.chrom.p, h->chrom, bytes, kind, c->copy_stream));
-    CU(cudaMemcpyAsync(s.a.p, h->a, bytes, kind, c->copy_stream));
-    CU(cudaMemcpyAsync(s.b.p, h->b, bytes, kind, c->copy_stream));
-    CU(cudaMemcpyAsync(s.rid.p, h->read_id, bytes, kind, c->copy_stream));
-    if (h->c) { CU(s.c.ensure(bytes)); CU(cudaMemcpyAsync(s.c.p, h->c, bytes, kind, c->copy_stream)); }
+    if (src.device && ((rc = SigTable::check_dev(c, *h, !contig_off)) || (rc = check_dev_col(c, contig_off, "contig_off")))) return rc;
+    if ((rc = upload_begin(c, src)) || (rc = s.size(h->n))) return rc;
+    if (contig_off && (rc = stage_group_offsets(c, t, contig_off, h->n, s.chrom.as<int32_t>(), src))) return rc;
+    if ((rc = s.copy_in(*h, !contig_off, src.kind(), c->copy_stream))) return rc;
     return upload_end(c, t, src);
 }
 extern "C" int csv_upload_sigs(csv_ctx* c, int t, const csv_sig_cols* h) { return upload_sigs_impl(c, t, h, nullptr, HOST_SRC); }
@@ -807,28 +947,16 @@ static int upload_reads_impl(csv_ctx* c, const csv_reads_cols* h, const int64_t*
     if (!c || !h) return set_err(CSV_E_INVALID, "bad argument");
     if (h->n < 0 || h->n >= (1ll << 31)) return set_err(CSV_E_INVALID, "read count out of range");
     CU(cudaSetDevice(c->device));
-    c->n_reads = h->n;
+    RowTable& r = c->reads;
+    r.n = h->n;
     inputs_replaced(c, CSV_NTYPES);
     if (h->n == 0) return CSV_OK;
-    if ((!contig_off && !h->chrom) || !h->start || !h->end || !h->read_id || !h->is_primary) return set_err(CSV_E_INVALID, "null column");
+    if (!RowTable::has_cols(*h, !contig_off)) return set_err(CSV_E_INVALID, "null column");
     int rc;
-    if (src.device) {
-        const void* col[6] = {contig_off ? nullptr : h->chrom, h->start, h->end, h->read_id, h->is_primary, contig_off};
-        static const char* const nm[6] = {"chrom", "start", "end", "read_id", "is_primary", "contig_off"};
-        for (int k = 0; k < 6; k++) if ((rc = check_dev_col(c, col[k], nm[k]))) return rc;
-    }
-    const size_t bytes = (size_t)h->n * 4;
-    const cudaMemcpyKind kind = src.kind();
-    rc = upload_begin(c, src);
-    if (rc) return rc;
-    CU(c->r_chrom.ensure(bytes)); CU(c->r_start.ensure(bytes)); CU(c->r_end.ensure(bytes)); CU(c->r_id.ensure(bytes));
-    CU(c->r_prim.ensure((size_t)h->n));
-    if (contig_off) { rc = stage_group_offsets(c, CSV_NTYPES, contig_off, h->n, c->r_chrom.as<int32_t>(), src); if (rc) return rc; }
-    else CU(cudaMemcpyAsync(c->r_chrom.p, h->chrom, bytes, kind, c->copy_stream));
-    CU(cudaMemcpyAsync(c->r_start.p, h->start, bytes, kind, c->copy_stream));
-    CU(cudaMemcpyAsync(c->r_end.p, h->end, bytes, kind, c->copy_stream));
-    CU(cudaMemcpyAsync(c->r_id.p, h->read_id, bytes, kind, c->copy_stream));
-    CU(cudaMemcpyAsync(c->r_prim.p, h->is_primary, (size_t)h->n, kind, c->copy_stream));
+    if (src.device && ((rc = RowTable::check_dev(c, *h, !contig_off)) || (rc = check_dev_col(c, contig_off, "contig_off")))) return rc;
+    if ((rc = upload_begin(c, src)) || (rc = r.size(h->n))) return rc;
+    if (contig_off && (rc = stage_group_offsets(c, CSV_NTYPES, contig_off, h->n, r.chrom.as<int32_t>(), src))) return rc;
+    if ((rc = r.copy_in(*h, !contig_off, src.kind(), c->copy_stream))) return rc;
     return upload_end(c, CSV_NTYPES, src);
 }
 
@@ -845,26 +973,25 @@ extern "C" int csv_upload_reads_grouped_device(csv_ctx* c, const csv_reads_cols*
     return upload_reads_impl(c, d, contig_off, UpSrc{true, (cudaStream_t)stream});
 }
 
-// Contig index (off, span: n_contigs + 2 entries) + sortedness check of the n rows of an alignment table (BAM order is a
-// precondition of the early-exit scan); one synchronisation.  A failure of the ctx's own table (c->a_*) leaves no table.
-static int aln_index(csv_ctx* c, int64_t n, const DBuf& chrom, const DBuf& start, const DBuf& end, DBuf& off, DBuf& span) {
+// Contig index (off, span: n_contigs + 2 entries) + sortedness check of the rows of an alignment table (BAM order is a
+// precondition of the early-exit scan); one synchronisation.  A failure leaves the table empty.
+static int aln_index(csv_ctx* c, AlnTable& t) {
     CU(c->aln_flag.ensure(64));
     uint32_t* flag = c->aln_flag.as<uint32_t>();
     CU(cudaMemsetAsync(flag, 0, 4, c->stream));
-    CU(cudaMemsetAsync(span.p, 0, ((size_t)c->n_contigs + 2) * 4, c->stream));
-    LAUNCH(c, c->stream, k_aln_index, grid_for(c, n, 256), 256, 0, chrom.as<int32_t>(), start.as<int32_t>(), end.as<int32_t>(), n,
-           c->n_contigs, span.as<int32_t>(), flag);
-    LAUNCH(c, c->stream, k_aln_off, grid_for(c, (int64_t)c->n_contigs + 1, 256), 256, 0, chrom.as<int32_t>(), n, c->n_contigs, off.as<uint32_t>());
+    CU(cudaMemsetAsync(t.span.p, 0, ((size_t)c->n_contigs + 2) * 4, c->stream));
+    LAUNCH(c, c->stream, k_aln_index, grid_for(c, t.n, 256), 256, 0, t.chrom.as<int32_t>(), t.start.as<int32_t>(), t.end.as<int32_t>(), t.n,
+           c->n_contigs, t.span.as<int32_t>(), flag);
+    LAUNCH(c, c->stream, k_aln_off, grid_for(c, (int64_t)c->n_contigs + 1, 256), 256, 0, t.chrom.as<int32_t>(), t.n, c->n_contigs, t.off.as<uint32_t>());
     uint32_t hflag = 0;
     CU(cudaMemcpyAsync(&hflag, flag, 4, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     if (hflag) {
-        if (&chrom == &c->a_chrom) c->n_aln = 0;
+        t.n = 0;
         return set_err(CSV_E_INPUT, "alignment table: %s", (hflag & ST_UNSORTED) ? "not coordinate-sorted (BAM order required)" : "contig id out of range");
     }
     return CSV_OK;
 }
-static int aln_index(csv_ctx* c, int64_t n) { return aln_index(c, n, c->a_chrom, c->a_start, c->a_end, c->a_off, c->a_span); }
 
 // The alignment table is copied on the ctx stream and its order is checked before the call returns (one synchronisation, for host
 // and device columns alike), so a device source's buffers are free again on return.
@@ -873,33 +1000,23 @@ static int upload_alignments_impl(csv_ctx* c, const csv_reads_cols* h, const UpS
     if (c->n_contigs == 0) return set_err(CSV_E_STATE, "csv_set_contigs has not been called");
     if (h->n < 0 || h->n >= (1ll << 31)) return set_err(CSV_E_INVALID, "alignment count out of range");
     CU(cudaSetDevice(c->device));
-    c->n_aln = h->n;
+    AlnTable& A = c->aln;
+    A.n = h->n;
     c->counts_valid = false;
     if (kind_scanned(c->ex.kind)) c->ex.kind = PacketKind::NAMED;   // the table no longer comes from a scanned accumulation
-    c->ex.n_pending = 0;
+    c->ex.pending.n = 0;
     if (h->n == 0) return CSV_OK;
-    if (!h->chrom || !h->start || !h->end || !h->read_id || !h->is_primary) return set_err(CSV_E_INVALID, "null column");
-    if (src.device) {
-        const void* col[5] = {h->chrom, h->start, h->end, h->read_id, h->is_primary};
-        static const char* const nm[5] = {"chrom", "start", "end", "read_id", "is_primary"};
-        for (int k = 0; k < 5; k++) { int rc = check_dev_col(c, col[k], nm[k]); if (rc) return rc; }
-    }
-    const size_t bytes = (size_t)h->n * 4;
-    const cudaMemcpyKind kind = src.kind();
-    CU(c->a_chrom.ensure(bytes)); CU(c->a_start.ensure(bytes)); CU(c->a_end.ensure(bytes)); CU(c->a_id.ensure(bytes));
-    CU(c->a_prim.ensure((size_t)h->n));
-    CU(c->a_off.ensure(((size_t)c->n_contigs + 2) * 4)); CU(c->a_span.ensure(((size_t)c->n_contigs + 2) * 4));
+    if (!RowTable::has_cols(*h, true)) return set_err(CSV_E_INVALID, "null column");
+    int rc;
+    if (src.device && (rc = RowTable::check_dev(c, *h, true))) return rc;
+    if ((rc = A.size(h->n)) || (rc = A.size_index(c->n_contigs))) return rc;
     CU(c->counters.ensure(sizeof(Counters)));
     if (src.device) {
         CU(cudaEventRecord(c->ev_prod, src.producer));
         CU(cudaStreamWaitEvent(c->stream, c->ev_prod, 0));
     }
-    CU(cudaMemcpyAsync(c->a_chrom.p, h->chrom, bytes, kind, c->stream));
-    CU(cudaMemcpyAsync(c->a_start.p, h->start, bytes, kind, c->stream));
-    CU(cudaMemcpyAsync(c->a_end.p, h->end, bytes, kind, c->stream));
-    CU(cudaMemcpyAsync(c->a_id.p, h->read_id, bytes, kind, c->stream));
-    CU(cudaMemcpyAsync(c->a_prim.p, h->is_primary, (size_t)h->n, kind, c->stream));
-    return aln_index(c, h->n);
+    if ((rc = A.copy_in(*h, true, src.kind(), c->stream))) return rc;
+    return aln_index(c, A);
 }
 extern "C" int csv_upload_alignments(csv_ctx* c, const csv_reads_cols* h) { return upload_alignments_impl(c, h, HOST_SRC); }
 extern "C" int csv_upload_alignments_device(csv_ctx* c, const csv_reads_cols* d, void* stream) {
@@ -1103,7 +1220,7 @@ static int run_segment_and_cluster(csv_ctx* c, Lane& L, TypeJob& J, int t, uint3
 }
 
 static int run_indel(csv_ctx* c, Lane& L, int t, uint32_t kslot_base) {
-    SigBuf& s = c->sig[t];
+    SigTable& s = c->sig[t];
     const cudaStream_t st = L.stream;
     const int64_t n = s.n;
     const uint64_t total = c->contig_off[c->n_contigs];
@@ -1206,7 +1323,7 @@ static int run_indel(csv_ctx* c, Lane& L, int t, uint32_t kslot_base) {
 }
 
 static int run_other(csv_ctx* c, Lane& L, int t, uint32_t kslot_base) {
-    SigBuf& s = c->sig[t];
+    SigTable& s = c->sig[t];
     const cudaStream_t st = L.stream;
     const int64_t n = s.n;
     SmallWork& w = L.small;
@@ -1420,7 +1537,7 @@ static int enqueue_cluster(csv_ctx* c, uint32_t type_mask) {
         Lane& L = c->lanes[lanes ? t : 0];
         if (&L != &c->lanes[0] && !L.used) { CU(cudaStreamWaitEvent(L.stream, c->ev_fork, 0)); L.used = true; }
         rc = wait_upload(c, L.stream, t);
-        if (!rc && c->up_checked[t]) LAUNCH(c, L.stream, k_fold_status, 1, 32, 0, c->up_status.as<uint32_t>() + t, &ctr->status);
+        if (!rc && c->up[t].checked) LAUNCH(c, L.stream, k_fold_status, 1, 32, 0, c->up_status.as<uint32_t>() + t, &ctr->status);
         if (!rc) rc = (t == CSV_DEL || t == CSV_INS) ? run_indel(c, L, t, kslot_base) : run_other(c, L, t, kslot_base);
         if (rc) {   // the ctx stream must not run ahead of work already forked
             join_lanes(c);
@@ -1480,7 +1597,7 @@ static int enqueue_cluster(csv_ctx* c, uint32_t type_mask) {
     // ---- genotype ----
     rc = wait_upload(c, c->stream, CSV_NTYPES);
     if (rc) return rc;
-    if (c->up_checked[CSV_NTYPES] && c->n_reads > 0)
+    if (c->up[CSV_NTYPES].checked && c->reads.n > 0)
         LAUNCH(c, c->stream, k_fold_status, 1, 32, 0, c->up_status.as<uint32_t>() + CSV_NTYPES, &ctr->status);
     stage_begin(c, c->stream, CSV_ST_GENOTYPE);
     {
@@ -1493,31 +1610,29 @@ static int enqueue_cluster(csv_ctx* c, uint32_t type_mask) {
             LAUNCH_PDL(c, c->stream, (k_scan_excl<4>), grid_for(c, G.n_bins + 1, SEL_THREADS * 4, 4), SEL_THREADS, 0, G.bin_start, (int64_t)G.n_bins + 1,
                    (const uint32_t*)nullptr, (const uint32_t*)nullptr, (uint32_t*)nullptr, ts);
             LAUNCH_PDL(c, c->stream, (k_windows<1>), grid_for(c, c->cap_cand, 256, 4), 256, 0, G);
-            if (c->n_reads > 0) {
+            if (c->reads.n > 0) {
+                const GcReads R = c->reads.gc_reads();
                 PairBuf PB;
-                PB.cap = (uint32_t)std::min<int64_t>(4 * c->n_reads + (1 << 20), (int64_t)1 << 30);
+                PB.cap = (uint32_t)std::min<int64_t>(4 * R.n + (1 << 20), (int64_t)1 << 30);
                 if (c->pair_cap_override > 0) PB.cap = (uint32_t)c->pair_cap_override;  // tests: force the overflow path
                 CU(c->pairs.ensure((size_t)PB.cap * (G.lin32 ? sizeof(uint4) : sizeof(uint2))));
                 PB.pairs = c->pairs.as<uint2>();
                 PB.pairs4 = c->pairs.as<uint4>();
                 PB.count = &ctr->n_windows;
                 if (G.lin32) {
-                    LAUNCH_PDL(c, c->stream, (k_reads_pass<true>), std::min(grid_for(c, c->n_reads, 1024, 8), resident_grid(c, k_reads_pass<true>, 256, 0)), 256, 0, G, PB, c->r_chrom.as<int32_t>(), c->r_start.as<int32_t>(),
-                           c->r_end.as<int32_t>(), c->r_id.as<int32_t>(), c->r_prim.as<uint8_t>(), c->n_reads, &ctr->status);
-                    LAUNCH_PDL(c, c->stream, (k_pairs_test<true>), c->n_sm * 8, 256, 0, G, PB, c->r_chrom.as<int32_t>(), c->r_start.as<int32_t>(),
-                           c->r_end.as<int32_t>(), c->r_id.as<int32_t>());
+                    LAUNCH_PDL(c, c->stream, (k_reads_pass<true>), std::min(grid_for(c, R.n, 1024, 8), resident_grid(c, k_reads_pass<true>, 256, 0)), 256, 0, G, PB,
+                               R.chrom, R.start, R.end, R.rid, R.prim, R.n, &ctr->status);
+                    LAUNCH_PDL(c, c->stream, (k_pairs_test<true>), c->n_sm * 8, 256, 0, G, PB, R.chrom, R.start, R.end, R.rid);
                 } else {
-                    LAUNCH_PDL(c, c->stream, (k_reads_pass<false>), std::min(grid_for(c, c->n_reads, 1024, 8), resident_grid(c, k_reads_pass<false>, 256, 0)), 256, 0, G, PB, c->r_chrom.as<int32_t>(), c->r_start.as<int32_t>(),
-                           c->r_end.as<int32_t>(), c->r_id.as<int32_t>(), c->r_prim.as<uint8_t>(), c->n_reads, &ctr->status);
-                    LAUNCH_PDL(c, c->stream, (k_pairs_test<false>), c->n_sm * 8, 256, 0, G, PB, c->r_chrom.as<int32_t>(), c->r_start.as<int32_t>(),
-                           c->r_end.as<int32_t>(), c->r_id.as<int32_t>());
+                    LAUNCH_PDL(c, c->stream, (k_reads_pass<false>), std::min(grid_for(c, R.n, 1024, 8), resident_grid(c, k_reads_pass<false>, 256, 0)), 256, 0, G, PB,
+                               R.chrom, R.start, R.end, R.rid, R.prim, R.n, &ctr->status);
+                    LAUNCH_PDL(c, c->stream, (k_pairs_test<false>), c->n_sm * 8, 256, 0, G, PB, R.chrom, R.start, R.end, R.rid);
                 }
             }
         }
         LAUNCH_PDL(c, c->stream, k_finalize, grid_for(c, c->cap_cand, 256, 4), 256, 0, G);
-        if (c->P.genotype && c->n_aln > 0 && (type_mask >> CSV_TRA & 1) && c->sig[CSV_TRA].n > 0) {
-            AlnView A{c->a_chrom.as<int32_t>(), c->a_start.as<int32_t>(), c->a_end.as<int32_t>(), c->a_id.as<int32_t>(), c->a_prim.as<uint8_t>(),
-                      c->a_off.as<uint32_t>(), c->a_span.as<int32_t>(), c->d_len.as<int64_t>()};
+        if (c->P.genotype && c->aln.n > 0 && (type_mask >> CSV_TRA & 1) && c->sig[CSV_TRA].n > 0) {
+            const AlnView A = c->aln.view(c->d_len.as<int64_t>());
             LAUNCH(c, c->stream, k_tra_genotype, c->n_sm * 8, 128, 0, G, A, c->P.bias_tra, c->P.gt_round);   // 4 warps per CTA, one warp per TRA candidate
         }
     }
@@ -1549,8 +1664,8 @@ extern "C" int csv_cluster(csv_ctx* c, uint32_t type_mask) {
     // uploads keep their per-type waits, which let the H2D copies of later types overlap the kernels of earlier ones.
     bool pending = false;
     for (int t = 0; t <= CSV_NTYPES; t++) {
-        if (c->up_pending[t] && c->up_device[t]) { rc = wait_upload(c, c->stream, t); if (rc) return rc; }
-        pending |= c->up_pending[t];
+        if (c->up[t].pending && c->up[t].device) { rc = wait_upload(c, c->stream, t); if (rc) return rc; }
+        pending |= c->up[t].pending;
     }
     bool done = false;
     if (c->graphs_enabled && !c->profiling && !c->lane_marks && !pending) {
@@ -1558,8 +1673,8 @@ extern "C" int csv_cluster(csv_ctx* c, uint32_t type_mask) {
         memset(&key, 0, sizeof(key));
         key.mask = type_mask;
         for (int t = 0; t < CSV_NTYPES; t++) { key.n[t] = c->sig[t].n; key.small_chain[t] = c->small_chain[t]; }
-        for (int t = 0; t <= CSV_NTYPES; t++) key.up_checked[t] = c->up_checked[t];
-        key.n_reads = c->n_reads; key.n_aln = c->n_aln; key.P = c->P; key.lanes = c->lanes_enabled ? 1 : 0;
+        for (int t = 0; t <= CSV_NTYPES; t++) key.up_checked[t] = c->up[t].checked;
+        key.n_reads = c->reads.n; key.n_aln = c->aln.n; key.P = c->P; key.lanes = c->lanes_enabled ? 1 : 0;
         key.alloc_epoch = g_alloc_epoch.load(); key.cfg_epoch = c->cfg_epoch;
         csv_ctx::GraphSlot* hit = nullptr;
         for (auto& g : c->graphs) if (g.valid && key_equal(g.key, key)) hit = &g;
