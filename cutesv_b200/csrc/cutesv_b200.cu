@@ -321,7 +321,7 @@ struct Lane {
     bool prev_is_chain_kernel = false;  // the launch being enqueued directly follows a chain kernel on this stream
     int mark = -1;                      // lane_marks: index of the open back-end interval in kivs
     DBuf keys_a, keys_b, vals_a, vals_b, hist, lb_status, big_list, giant_list, giant_arena;
-    DBuf boff, rec_a, recc_a, rest_list;   // partitioned INS/DEL front end, k_cluster_small's rest list
+    DBuf boff, rec_a, recc_a, rest_list;   // partitioned INS/DEL front end (edge counts | page table), k_cluster_small's rest list
     SmallWork small;
 };
 static constexpr int N_LANES = CSV_NTYPES;
@@ -1242,36 +1242,43 @@ static int run_indel(csv_ctx* c, Lane& L, int t, uint32_t kslot_base) {
     uint32_t* sidx = nullptr;
     int rc;
     if (prefilter) {
-        // filter-first front end, partitioned by genome range: scatter of (key, index) by partition inside every round of
-        // PART_ROUND rows -> per partition, in shared memory, over its runs: bucket histogram, density flags, survivors in
+        // filter-first front end, partitioned by genome range: scatter of (key, index) by partition into each partition's
+        // pages of a pool -> per partition, in shared memory, over its pages: bucket histogram, density flags, survivors in
         // key order.  W: the widest partitions (at most 2^22 bp) that still give every SM about two of them.
         int W = PART_W_MAX;
         while (W > PART_W_MIN && (int64_t)(total >> W) + 1 < 2 * (int64_t)c->n_sm) W--;
         const int P = (int)(total >> W) + 1;
         const int n_chunks = (int)((n + PART_ROUND - 1) / PART_ROUND);
-        const size_t run_words = (size_t)(P + 1) * n_chunks, edge_words = (size_t)P * 2 * BKT_PAD;
+        const uint32_t ptw = (uint32_t)((n + PART_PAGE - 1) / PART_PAGE) + 1;   // page-table row: every page of n pairs, + 1
+        // edge counts at a fixed size in front, so that the fill counters and page table behind them, all zero between
+        // calls, stay zero whatever P and n the next call has
+        const size_t edge_words = (size_t)PART_MAX * 2 * BKT_PAD, tab_words = PART_MAX + (size_t)P * ptw;
         stage_begin(c, st, CSV_ST_KEYS);
-        CU(L.boff.ensure((run_words + edge_words) * 4));   // run table (P + 1 rows of n_chunks) | edges
-        uint32_t* runs = L.boff.as<uint32_t>();
-        uint32_t* edge = runs + run_words;
+        CU(L.boff.ensure((edge_words + tab_words) * 4, true));   // edges | fill[PART_MAX] | pt[P][ptw]
+        uint32_t* edge = L.boff.as<uint32_t>();
+        uint32_t* fill = edge + edge_words;
+        uint32_t* pt = fill + PART_MAX;
+        CU(L.keys_a.ensure(((size_t)ptw - 1 + P) * PART_PAGE * 8));   // the page pool
+        uint2* pool = (uint2*)L.keys_a.p;
         // the spill area of partitions whose survivors exceed the shared-memory stage; the member records use it later
         CU(L.rec_a.ensure((size_t)n * sizeof(IndelRec)));
-        CU(cudaMemsetAsync(edge, 0, edge_words * 4, st));
+        CU(cudaMemsetAsync(edge, 0, (size_t)P * 2 * BKT_PAD * 4, st));
         const int is_ins = t == CSV_INS ? 1 : 0;
         if ((((uintptr_t)s.chrom.p) | ((uintptr_t)s.a.p)) & 15)   // k_part_scatter loads both columns 16 B at a time
             return set_err(CSV_E_STATE, "signature columns are not 16 B aligned");
-        uint2* pairs = (uint2*)L.keys_a.p;   // 8 B per signature (ensure_lane_scratch)
-        LAUNCH(c, st, k_part_scatter, n_chunks, PS_THREADS, ps_smem_bytes(), s.chrom.as<int32_t>(), s.a.as<int32_t>(), n, is_ins, ct, W, P,
-               n_chunks, rb, pairs, runs, edge, &ctr->status);
-        stage_end(c, st, CSV_ST_KEYS);
-        stage_begin(c, st, CSV_ST_SORT);
+        // Everything that can fail on the host is done before the scatter: once it is enqueued, its filter is enqueued
+        // right behind it, and the filter resets the fill counters and page-table entries the scatter set.
+        uint32_t* pool_next = nullptr;   // zeroed by k_begin
         TileSync ts;
-        rc = make_sync(c->lb, L.lb_status, st, (size_t)P, &ts);
-        if (rc) return rc;
-        uint32_t* n_pass = &ctr->n_dom[t];
+        if ((rc = take_ticket(c->lb, &pool_next)) || (rc = make_sync(c->lb, L.lb_status, st, (size_t)P, &ts))) return rc;
         const size_t smem = pf_smem_bytes(W);
         const int g = std::min(P, resident_grid(c, k_part_filter, 256, smem));
-        LAUNCH_PDL(c, st, k_part_filter, g, 256, smem, (const uint2*)pairs, (const uint32_t*)runs, n_chunks, P, W, rb, (uint32_t)J.cp.min_support,
+        LAUNCH(c, st, k_part_scatter, n_chunks, PS_THREADS, ps_smem_bytes(), s.chrom.as<int32_t>(), s.a.as<int32_t>(), n, is_ins, ct, W, P,
+               rb, pool, fill, pt, ptw, pool_next, edge, &ctr->status);
+        stage_end(c, st, CSV_ST_KEYS);
+        stage_begin(c, st, CSV_ST_SORT);
+        uint32_t* n_pass = &ctr->n_dom[t];
+        LAUNCH_PDL(c, st, k_part_filter, g, 256, smem, (const uint2*)pool, fill, pt, ptw, P, W, rb, (uint32_t)J.cp.min_support,
                    (const uint32_t*)edge, L.keys_b.as<uint32_t>(), L.vals_b.as<uint32_t>(), (uint2*)L.rec_a.p, n_pass, ts);
         stage_end(c, st, CSV_ST_SORT);
         if (c->lane_marks) {

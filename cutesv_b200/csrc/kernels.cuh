@@ -365,11 +365,11 @@ __device__ __forceinline__ uint32_t indel_key32(int32_t c, int32_t raw, int is_i
 // INS / DEL front end, partitioned: the genome's linear coordinate is cut into P partitions of 2^W bp (W <= 22, so a
 // partition has at most 16384 buckets of 256 bp).  The density filter then needs no genome-sized bucket table: every
 // partition's histogram is built, flagged, scanned and used inside one CTA's shared memory.
-//    k_part_scatter  8 B/sig read (chrom, a),        -> per round of PART_ROUND rows: its (key, index) pairs grouped by
-//                    8 B/sig written                    partition, written in place; the round's partition offsets (the
-//                                                       run table); halo counts at partition edges; input validation
-//    k_part_filter   8 B/sig read (twice, the second  -> survivors in key order, 8 B per survivor written
-//                    mostly from L2) + the run table
+//    k_part_scatter  8 B/sig read (chrom, a),        -> the (key, index) pairs, every partition's written to its own pages
+//                    8 B/sig written                    of a shared pool (fill counters, page table); halo counts at
+//                                                       partition edges; input validation
+//    k_part_filter   8 B/sig read (twice, the second  -> survivors in key order, 8 B per survivor written; the partition's
+//                    mostly from L2) + the page ids     fill counter and page-table entries reset
 // ------------------------------------------------------------------------------------------
 static constexpr int PART_MAX = 1024;        // partitions: 32-bit keys, W = 22
 static constexpr int PART_W_MAX = 22;
@@ -381,14 +381,24 @@ __host__ __device__ constexpr size_t pf_smem_bytes(int w) {
     return (size_t)(1u << (w - BKT_SHIFT)) * 4 + (size_t)(1u << (w - BKT_SHIFT)) / 32 * 4 + (size_t)PF_STAGE * 8;
 }
 
+// Paged partitions: the pairs of partition p take the ordinals 0 .. fill[p] - 1 of p, in pages of PART_PAGE pairs drawn
+// from one pool; pt[p * ptw + k] = 1 + the pool page that holds ordinals k * PART_PAGE .., 0 while the page is unassigned.
+// At most one page per partition is partly filled, so a pool of ceil(n / PART_PAGE) + P pages and rows of
+// ptw = ceil(n / PART_PAGE) + 1 entries always suffice.  Both fill and pt are all zero between calls: k_part_filter
+// resets every entry the scatter set.
+static constexpr int PART_PAGE = 2048;   // 16 KB of pairs
+static_assert(PART_PAGE % 2 == 0, "k_part_filter reads pairs two at a time, 16 B aligned");
+
 // One 1024-thread CTA per round of PART_ROUND rows (round c: rows c * PART_ROUND ..), one CTA per SM.  The round's
-// (key, row) pairs are grouped by partition in shared memory and written back in place, pairs[c * PART_ROUND + q], with
-// coalesced 16 B stores: partition p of round c is the run [runs[p * n_chunks + c], runs[(p + 1) * n_chunks + c]) of that
-// block (row P of the run table holds the round's row count).  The order inside a partition is irrelevant (k_part_filter
-// orders it), and the filter reads a partition as its list of runs, so no pass has to count the rows of every partition
-// before they are written.  The larger the round, the longer and fewer the runs the filter walks (config 2: 8.4 M rows of a
-// type, P = 741, about 22 pairs per partition and round).  16384 rows give 513 rounds of a type there, about 3.9 waves of
-// one CTA per SM on 132 SMs; 24576 rows (about 2.6 waves) made both kernels slower (DESIGN §5).
+// (key, row) pairs are grouped by partition in shared memory; thread p reserves the next cnt ordinals of partition p
+// (atomicAdd on fill[p]) and takes a pool page for every page that starts inside its reservation (one atomicAdd on the
+// pool counter), and publishes them in pt after the placement.  The page that holds its first ordinal, if that ordinal is
+// not a page start, belongs to the reservation before it: the thread then waits for that entry.  The wait cannot
+// deadlock: the owner's CTA reserved earlier, so it is resident or done, and no thread waits on another CTA before it
+// has published its own pages (only the CTA's own barriers lie between its reservation and its publication).  The grouped
+// round is then written out in order, position q (partition p) to ordinal resv[p] + q - run_off[p] of p, through the
+// page ids cached in shared memory, so a warp's stores stay consecutive within every run.  16384 rows give 513 rounds of
+// a type on config 2, about 3.9 waves of one CTA per SM on 132 SMs.
 // The round's `chrom` and `a` come in by two 1-D bulk copies on one mbarrier, into the shared memory that later holds the
 // grouped pairs; `chrom` and `a` must be 16 B aligned (run_indel checks it), and only the rows of the input's last
 // partial 4-row group are loaded row by row.  Every thread then reads its PART_ROUND_V 4-row groups with conflict-free
@@ -397,21 +407,27 @@ __host__ __device__ constexpr size_t pf_smem_bytes(int w) {
 // the halo of the neighbours' windows.
 static constexpr int PS_THREADS = 1024;
 static constexpr int PART_ROUND = 16384, PART_ROUND_V = PART_ROUND / 4 / PS_THREADS;   // 4-row groups per thread
-__host__ __device__ constexpr size_t ps_smem_bytes() { return (size_t)PART_ROUND * 8 + (size_t)PART_MAX * 4; }
+// pages one round touches: partition p's reservation of cnt rows spans at most cnt / PART_PAGE + 2 of them
+static constexpr int PS_PAGES = PART_ROUND / PART_PAGE + 2 * PART_MAX;
+__host__ __device__ constexpr size_t ps_smem_bytes() { return (size_t)PART_ROUND * 8 + (size_t)PART_MAX * 4 * 3 + (size_t)PS_PAGES * 4; }
 static_assert(PART_MAX == PS_THREADS && PART_ROUND % (4 * PS_THREADS) == 0, "k_part_scatter tiling: one partition per thread");
-// run offsets, row indices and c * PART_ROUND + offset are 32-bit (n < 2^32); one round must fit an SM's opt-in shared memory
+// run offsets, ordinals and row indices are 32-bit (n < 2^32); one round must fit an SM's opt-in shared memory
 static_assert(ps_smem_bytes() + 256 <= 227 * 1024, "k_part_scatter: one round per SM");
 __global__ void __launch_bounds__(PS_THREADS, 1) k_part_scatter(const int32_t* __restrict__ chrom, const int32_t* __restrict__ a, int64_t n,
-                                                                int is_ins, ContigTab ct, int W, int P, int n_chunks, int rb,
-                                                                uint2* __restrict__ pairs, uint32_t* __restrict__ runs,
-                                                                uint32_t* __restrict__ edge, uint32_t* status) {
+                                                                int is_ins, ContigTab ct, int W, int P, int rb, uint2* __restrict__ pool,
+                                                                uint32_t* __restrict__ fill, uint32_t* pt, uint32_t ptw,
+                                                                uint32_t* __restrict__ pool_next, uint32_t* __restrict__ edge,
+                                                                uint32_t* status) {
     pdl_launch_dependents();
     extern __shared__ __align__(16) uint32_t s_dyn[];
     uint2* s_st = reinterpret_cast<uint2*>(s_dyn);                   // PART_ROUND pairs, grouped by partition
     int32_t* s_c = reinterpret_cast<int32_t*>(s_dyn);                // before that: the round's chrom ..
     int32_t* s_a = reinterpret_cast<int32_t*>(s_dyn) + PART_ROUND;   // .. and a
     uint32_t* s_fill = s_dyn + 2 * PART_ROUND;   // rows of the round per partition -> next free position of it in s_st
-    __shared__ uint32_t s_warp[32];
+    uint32_t* s_d = s_fill + PART_MAX;           // partition p: ordinal - position in s_st (mod 2^32)
+    uint32_t* s_pb = s_d + PART_MAX;             // partition p: index in s_pg of its page k, minus k (mod 2^32)
+    uint32_t* s_pg = s_pb + PART_MAX;            // the pool pages of the round's reservations
+    __shared__ uint32_t s_warp[32], s_npg;
     __shared__ __align__(8) uint64_t s_bar;
     const int t = (int)threadIdx.x, lane = t & 31, warp = t >> 5;
     const int64_t s0 = (int64_t)blockIdx.x * PART_ROUND;
@@ -427,6 +443,7 @@ __global__ void __launch_bounds__(PS_THREADS, 1) k_part_scatter(const int32_t* _
         } else {
             mbar_arrive(&s_bar);
         }
+        s_npg = 0;
     }
     if (m4 + t < m) { s_c[m4 + t] = chrom[s0 + m4 + t]; s_a[m4 + t] = a[s0 + m4 + t]; }   // the input's last rows
     s_fill[t] = 0;
@@ -456,8 +473,11 @@ __global__ void __launch_bounds__(PS_THREADS, 1) k_part_scatter(const int32_t* _
         atomicAdd(&s_fill[p], 1u);
     }
     __syncthreads();   // every row counted, and read: the pairs may now overwrite the input
-    {   // exclusive scan of the per-partition counts, one partition per thread; the run table gets rows 0..P-1
-        const uint32_t v = s_fill[t];
+    // Reserve ordinals [r, r + v) of partition t (v > 0 only for t < P).  The latencies of the reservation, the page
+    // allocation and the first probe of the page-table entry of a page begun earlier run under the scan and the placement.
+    const uint32_t v = s_fill[t];
+    const uint32_t r = v ? atomicAdd(&fill[t], v) : 0u;
+    {   // exclusive scan of the per-partition counts, one partition per thread
         uint32_t incl = v;
 #pragma unroll
         for (int d = 1; d < 32; d <<= 1) {
@@ -479,74 +499,57 @@ __global__ void __launch_bounds__(PS_THREADS, 1) k_part_scatter(const int32_t* _
         __syncthreads();
         const uint32_t o = s_warp[warp] + incl - v;
         s_fill[t] = o;
-        if (t < P) runs[(int64_t)t * n_chunks + blockIdx.x] = o;
-        if (t == 0) runs[(int64_t)P * n_chunks + blockIdx.x] = (uint32_t)m;
+        s_d[t] = r - o;
     }
-    __syncthreads();
+    const uint32_t k0 = r / PART_PAGE, k1 = v ? (r + v - 1) / PART_PAGE : k0;
+    const bool lead = v && r % PART_PAGE != 0;   // page k0 was taken by an earlier reservation
+    const uint32_t np = v ? k1 - k0 + 1 : 0u, own = np - (lead ? 1u : 0u);
+    uint32_t* row = pt + (size_t)t * ptw;
+    const uint32_t id = own ? atomicAdd(pool_next, own) : 0u;
+    uint32_t g = 1;
+    if (lead) asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(g) : "l"(row + k0) : "memory");
+    uint32_t base = np;   // warp scan of the page counts -> this partition's slots in s_pg
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const uint32_t y = __shfl_up_sync(0xffffffffu, base, d);
+        if (lane >= d) base += y;
+    }
+    uint32_t wbase = 0;
+    if (lane == 31) wbase = atomicAdd(&s_npg, base);
+    base = __shfl_sync(0xffffffffu, wbase, 31) + base - np;
+    s_pb[t] = base - k0;
+    __syncthreads();   // s_fill holds the run offsets
 #pragma unroll
     for (int k = 0; k < 4 * PART_ROUND_V; k++) {
         const int q = 4 * ((k >> 2) * PS_THREADS + t) + (k & 3);
         if (q < m) s_st[atomicAdd(&s_fill[key[k] >> W], 1u)] = make_uint2(key[k], (uint32_t)(s0 + q));
     }
+    // publish this partition's pages, then (only then) wait for the page an earlier reservation began
+    for (uint32_t i = 0; i < own; i++) {
+        const uint32_t k = k1 + 1 - own + i;
+        asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(row + k), "r"(id + i + 1u) : "memory");
+        s_pg[base + k - k0] = id + i;
+    }
+    if (lead) {
+        while (g == 0) {
+            __nanosleep(64);
+            asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(g) : "l"(row + k0) : "memory");
+        }
+        s_pg[base] = g - 1u;
+    }
     __syncthreads();
-    uint2* dst = pairs + s0;   // 16 B aligned: s0 is a multiple of PART_ROUND
-    for (int q = t; q < (m >> 1); q += PS_THREADS) reinterpret_cast<uint4*>(dst)[q] = reinterpret_cast<const uint4*>(s_st)[q];
-    if ((m & 1) && t == 0) dst[m - 1] = s_st[m - 1];
-}
-
-// f(pair, valid) for every pair of partition p, i.e. of the runs [c * PART_ROUND + runs[p][c], c * PART_ROUND +
-// runs[p + 1][c]) of the rounds c < n_chunks (k_part_scatter's run table, runs[p][c] at runs[p * n_chunks + c]).  Every
-// warp takes tiles of TR consecutive runs, one per lane, in turn with the CTA's other warps (the next tile's run bounds are
-// loaded before the current one is walked).  TR = 32 when every warp gets at least two such tiles, else 16 (lanes TR..31
-// hold empty runs), so that a partition of few runs still spreads over all eight warps.  A warp scan of the run lengths
-// numbers the tile's pairs; the lane that takes pair e finds its run by a five-step binary search over the lanes' run ends
-// (shuffles: no shared memory, no per-pair search in memory).  U pairs per lane are loaded before f sees the first.  f is called by every lane of the warp
-// together, `valid` false past the tile's last pair.
-template <int U, class F>
-__device__ __forceinline__ void part_walk_runs(const uint2* __restrict__ pairs, const uint32_t* __restrict__ runs, int p, int n_chunks,
-                                               F f) {
-    const int lane = threadIdx.x & 31;
-    const uint32_t* r0 = runs + (int64_t)p * n_chunks;
-    const uint32_t* r1 = r0 + n_chunks;
-    const int TR = n_chunks >= 2 * 8 * 32 ? 32 : 16;
-    const bool mine = lane < TR;
-    int c = (int)(threadIdx.x >> 5) * TR + lane;   // warp w starts at run TR w
-    uint32_t nb = 0, ne = 0;
-    if (mine && c < n_chunks) { nb = __ldcg(r0 + c); ne = __ldcg(r1 + c); }
-    for (; c - lane < n_chunks; c += 8 * TR) {
-        const uint32_t len = ne - nb;
-        uint32_t end = len;   // inclusive scan of the run lengths: the tile's pairs end[r - 1] .. end[r] - 1 are run r's
 #pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const uint32_t v = __shfl_up_sync(0xffffffffu, end, d);
-            if (lane >= d) end += v;
-        }
-        const uint32_t tot = __shfl_sync(0xffffffffu, end, 31);
-        const uint32_t src = (uint32_t)c * PART_ROUND + nb - (end - len);   // pair e of the tile, in run r: pairs[src(r) + e]
-        nb = ne = 0;
-        if (mine && c + 8 * TR < n_chunks) { nb = __ldcg(r0 + c + 8 * TR); ne = __ldcg(r1 + c + 8 * TR); }
-        const uint32_t end15 = __shfl_sync(0xffffffffu, end, 15);   // the searches' first step
-        for (uint32_t e0 = 0; e0 < tot; e0 += 32 * U) {
-            uint32_t at[U];
-#pragma unroll
-            for (int u = 0; u < U; u++) {   // no branch around a search, so that the U searches interleave
-                const uint32_t e = e0 + 32 * u + lane;
-                int r = end15 <= e ? 16 : 0;
-#pragma unroll
-                for (int s = 8; s; s >>= 1) r += __shfl_sync(0xffffffffu, end, r + s - 1) <= e ? s : 0;
-                at[u] = __shfl_sync(0xffffffffu, src, r) + e;
-            }
-            uint2 pr[U];
-#pragma unroll
-            for (int u = 0; u < U; u++) pr[u] = e0 + 32 * u + lane < tot ? pairs[at[u]] : make_uint2(0u, 0u);
-#pragma unroll
-            for (int u = 0; u < U; u++) f(pr[u], e0 + 32 * u + lane < tot);
-        }
+    for (int j = 0; j < PART_ROUND / PS_THREADS; j++) {
+        const int q = j * PS_THREADS + t;
+        if (q >= m) break;
+        const uint2 pr = s_st[q];
+        const uint32_t p = pr.x >> W, e = (uint32_t)q + s_d[p];
+        pool[(size_t)s_pg[s_pb[p] + e / PART_PAGE] * PART_PAGE + e % PART_PAGE] = pr;
     }
 }
 
 // One partition per CTA iteration (partitions taken by ticket, in order):
-//   1. 256-bp bucket histogram of the partition in shared memory, its pairs read as the run list of the scatter's rounds
+//   1. 256-bp bucket histogram of the partition in shared memory, its pairs read from its pages (below)
 //   2. one pass over every thread's strip of BP / 256 consecutive buckets: keep flags by a sliding +-rb window (the halo
 //      taken from the neighbours' edge counts -- the same rule as a genome-wide histogram; strips whose windows stay
 //      inside the partition and reach only the neighbouring strips skip the halo tests) and the strip's survivors;
@@ -560,8 +563,12 @@ __device__ __forceinline__ void part_walk_runs(const uint2* __restrict__ pairs, 
 // threads reading the j-th bucket of their strips touch 256 consecutive words.  The look-back's exclusive base is
 // awaited only where it is used: before the placement of a partition that spills, otherwise by warp 0 before its share
 // of the placement, while the other warps place theirs.
-__global__ void __launch_bounds__(256) k_part_filter(const uint2* __restrict__ pairs, const uint32_t* __restrict__ runs, int n_chunks, int P, int W, int rb,
-                                                     uint32_t need, const uint32_t* __restrict__ edge, uint32_t* __restrict__ keys_out,
+// Both passes read the partition's ordinals e = 2 * thread, 2 * thread + 512, .. two pairs (16 B) at a time, U loads in
+// flight per thread: pool page pt[p][e / PART_PAGE] - 1, slot e % PART_PAGE.  The page ids are read through L1: row p of
+// the page table is read and reset by this CTA only.  Once both passes are done the CTA zeroes fill[p] and the entries
+// of row p it read, which are exactly the ones the scatter set, so the next call starts from a clean table.
+__global__ void __launch_bounds__(256) k_part_filter(const uint2* __restrict__ pool, uint32_t* __restrict__ fill, uint32_t* __restrict__ pt,
+                                                     uint32_t ptw, int P, int W, int rb, uint32_t need, const uint32_t* __restrict__ edge, uint32_t* __restrict__ keys_out,
                                                      uint32_t* __restrict__ idx_out, uint2* __restrict__ spill, uint32_t* n_out, TileSync ts) {
     pdl_launch_dependents(); pdl_wait();
     extern __shared__ __align__(16) uint32_t s_dyn[];
@@ -592,12 +599,32 @@ __global__ void __launch_bounds__(256) k_part_filter(const uint2* __restrict__ p
             const bool ok = q >= 0 && q < P && j < rb;
             (right ? s_hr : s_hl)[j] = ok ? edge[(int64_t)q * 2 * BKT_PAD + (right ? 0 : BKT_PAD) + j] : 0u;
         }
-        // 1. histogram (the partition's pairs are the runs of the scatter's rounds)
-        constexpr int U = 16;   // loads in flight per thread: a tile of 32 runs (about 700 pairs at W = 22) in two round trips
-                                // (24 was no faster, DESIGN §5)
-        part_walk_runs<U>(pairs, runs, p, n_chunks, [&](uint2 pr, bool v) {
-            if (v) atomicAdd(&s_h[phys((pr.x >> BKT_SHIFT) & bmask)], 1u);
-        });
+        const uint32_t np = __ldcg(fill + p);
+        uint32_t* row = pt + (size_t)p * ptw;
+        auto walk = [&](auto f) {
+            constexpr int U = 8;   // 16 B loads in flight per thread: a step of the CTA covers pages k and k + 1 exactly
+            static_assert(2 * 256 * U == 2 * PART_PAGE, "k_part_filter: two pages per step");
+            for (uint32_t k = 0; 2 * PART_PAGE * k < np; k++) {
+                const uint32_t e0 = 2 * PART_PAGE * k + 2 * threadIdx.x;
+                const uint2* pg0 = pool + (size_t)(__ldg(row + 2 * k) - 1u) * PART_PAGE;
+                const uint2* pg1 = PART_PAGE * (2 * k + 1) < np ? pool + (size_t)(__ldg(row + 2 * k + 1) - 1u) * PART_PAGE : pg0;
+                uint4 v[U];
+#pragma unroll
+                for (int u = 0; u < U; u++) {
+                    const uint32_t e = e0 + 2 * 256 * u;
+                    v[u] = e < np ? __ldg(reinterpret_cast<const uint4*>((2 * 256 * u + 2 * threadIdx.x < PART_PAGE ? pg0 : pg1) + e % PART_PAGE))
+                                  : make_uint4(0u, 0u, 0u, 0u);
+                }
+#pragma unroll
+                for (int u = 0; u < U; u++) {
+                    const uint32_t e = e0 + 2 * 256 * u;
+                    if (e < np) f(make_uint2(v[u].x, v[u].y));
+                    if (e + 1 < np) f(make_uint2(v[u].z, v[u].w));
+                }
+            }
+        };
+        // 1. histogram
+        walk([&](uint2 pr) { atomicAdd(&s_h[phys((pr.x >> BKT_SHIFT) & bmask)], 1u); });
         __syncthreads();
         // 2. keep flags of the strip, the partition's survivor total and the strip's first slot.  Interior strips read the
         // transposed histogram straight: bucket b0 + s * PER + j of the strip s = -1, 0, 1 is at (j << 8) + thread + s.
@@ -632,11 +659,13 @@ __global__ void __launch_bounds__(256) k_part_filter(const uint2* __restrict__ p
         }
         uint2* st = spilled ? spill + s_excl : s_st;
         // 3b. survivors into their buckets' slot ranges (afterwards s_h[phys(b)] = end of bucket b)
-        part_walk_runs<U>(pairs, runs, p, n_chunks, [&](uint2 pr, bool v) {
+        walk([&](uint2 pr) {
             const uint32_t ph = phys((pr.x >> BKT_SHIFT) & bmask);
-            if (v && ((s_f[ph >> 5] >> (ph & 31)) & 1u)) st[atomicAdd(&s_h[ph], 1u)] = pr;
+            if ((s_f[ph >> 5] >> (ph & 31)) & 1u) st[atomicAdd(&s_h[ph], 1u)] = pr;
         });
-        __syncthreads();
+        __syncthreads();   // every page id and pair read
+        for (uint32_t k = threadIdx.x; k < (np + PART_PAGE - 1) / PART_PAGE; k += 256) row[k] = 0u;
+        if (threadIdx.x == 0) fill[p] = 0u;
         const uint32_t obase = s_excl;
         // 4a. small buckets: rank against the bucket, ties by slot
         for (uint32_t q = threadIdx.x; q < S; q += 256) {
