@@ -1262,7 +1262,7 @@ CSV_HD uint32_t pf_count(const H& h, int k, int bp, const uint32_t* hl, const ui
 CSV_HD bool pf_strip_interior(int b0, int n, int bp, int rb) { return rb <= n && b0 - rb >= 0 && b0 + n - 1 + rb < bp; }
 
 // pf_strip_flags of an interior strip.  hs(s, j) = h(b0 + s * n + j) for s = -1, 0, 1 and 0 <= j < n: the caller indexes
-// its histogram directly (k_part_filter's transposed histogram: word (j << 8) + thread + s).
+// its histogram directly (k_part_filter's transposed histogram: word (j << 9) + thread + s).
 template <class HS>
 CSV_HD uint64_t pf_strip_flags_interior(const HS& hs, int n, int rb, uint32_t need, uint32_t* kept) {
     uint32_t win = 0, sum = 0;

@@ -1272,13 +1272,13 @@ static int run_indel(csv_ctx* c, Lane& L, int t, uint32_t kslot_base) {
         TileSync ts;
         if ((rc = take_ticket(c->lb, &pool_next)) || (rc = make_sync(c->lb, L.lb_status, st, (size_t)P, &ts))) return rc;
         const size_t smem = pf_smem_bytes(W);
-        const int g = std::min(P, resident_grid(c, k_part_filter, 256, smem));
+        const int g = std::min(P, resident_grid(c, k_part_filter, PF_THREADS, smem));
         LAUNCH(c, st, k_part_scatter, n_chunks, PS_THREADS, ps_smem_bytes(), s.chrom.as<int32_t>(), s.a.as<int32_t>(), n, is_ins, ct, W, P,
                rb, pool, fill, pt, ptw, pool_next, edge, &ctr->status);
         stage_end(c, st, CSV_ST_KEYS);
         stage_begin(c, st, CSV_ST_SORT);
         uint32_t* n_pass = &ctr->n_dom[t];
-        LAUNCH_PDL(c, st, k_part_filter, g, 256, smem, (const uint2*)pool, fill, pt, ptw, P, W, rb, (uint32_t)J.cp.min_support,
+        LAUNCH_PDL(c, st, k_part_filter, g, PF_THREADS, smem, (const uint2*)pool, fill, pt, ptw, P, W, rb, (uint32_t)J.cp.min_support,
                    (const uint32_t*)edge, L.keys_b.as<uint32_t>(), L.vals_b.as<uint32_t>(), (uint2*)L.rec_a.p, n_pass, ts);
         stage_end(c, st, CSV_ST_SORT);
         if (c->lane_marks) {

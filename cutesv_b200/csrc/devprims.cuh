@@ -115,9 +115,12 @@ __device__ __forceinline__ uint32_t lookback_exclusive_warp(uint64_t* status, ui
     return lookback_wait_warp(status, gen, tile, local);
 }
 
-// exclusive scan of one value per thread across a 256-thread CTA; returns exclusive prefix,
-// *total = CTA sum.  s_warp: 9 words of shared memory.
-__device__ __forceinline__ uint32_t block_excl_scan_256(uint32_t v, uint32_t* s_warp, uint32_t* total) {
+// exclusive scan of one value per thread across an NT-thread CTA (NT = 64 .. 1024, a multiple of 32); returns exclusive
+// prefix, *total = CTA sum.  s_warp: NT / 32 + 1 words of shared memory.
+template <int NT>
+__device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t* s_warp, uint32_t* total) {
+    static_assert(NT % 32 == 0 && NT >= 64 && NT <= 1024, "block_excl_scan: whole warps, at most 32");
+    constexpr int NW = NT / 32;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     uint32_t incl = v;
 #pragma unroll
@@ -128,19 +131,19 @@ __device__ __forceinline__ uint32_t block_excl_scan_256(uint32_t v, uint32_t* s_
     if (lane == 31) s_warp[warp] = incl;
     __syncthreads();
     if (warp == 0) {
-        uint32_t w = lane < 8 ? s_warp[lane] : 0;
+        uint32_t w = lane < NW ? s_warp[lane] : 0;
         uint32_t wi = w;
 #pragma unroll
-        for (int d = 1; d < 8; d <<= 1) {
+        for (int d = 1; d < NW; d <<= 1) {
             uint32_t y = __shfl_up_sync(0xffffffffu, wi, d);
             if (lane >= d) wi += y;
         }
-        if (lane < 8) s_warp[lane] = wi - w;
-        if (lane == 7) s_warp[8] = wi;
+        if (lane < NW) s_warp[lane] = wi - w;
+        if (lane == NW - 1) s_warp[NW] = wi;
     }
     __syncthreads();
     uint32_t r = s_warp[warp] + incl - v;
-    *total = s_warp[8];
+    *total = s_warp[NW];
     __syncthreads();
     return r;
 }
@@ -222,7 +225,7 @@ __global__ void __launch_bounds__(SEL_THREADS) k_select(Pred pred, int64_t n_hos
             if (i < n && pred(i)) { flags |= 1u << j; cnt++; }
         }
         uint32_t total;
-        const uint32_t local = block_excl_scan_256(cnt, s_warp, &total);
+        const uint32_t local = block_excl_scan<256>(cnt, s_warp, &total);
         if (threadIdx.x < 32) {
             const uint32_t ex = lookback_exclusive_warp(ts.status, gen, (int)tile, total);
             if (threadIdx.x == 0) {
@@ -283,7 +286,7 @@ __global__ void __launch_bounds__(SEL_THREADS) k_scan_excl(uint32_t* arr, int64_
             }
         }
         uint32_t total;
-        const uint32_t local = block_excl_scan_256(cnt, s_warp, &total);
+        const uint32_t local = block_excl_scan<256>(cnt, s_warp, &total);
         if (threadIdx.x < 32) {
             const uint32_t ex = lookback_exclusive_warp(ts.status, gen, (int)tile, total);
             if (threadIdx.x == 0) {

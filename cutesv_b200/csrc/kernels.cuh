@@ -171,7 +171,7 @@ __global__ void __launch_bounds__(SEL_THREADS) k_select_heads(TypeJob J, uint32_
             if (base + p < n && chain_head(s_link, q0 + p, need)) { flags |= 1u << j; cnt++; }
         }
         uint32_t total;
-        const uint32_t local = block_excl_scan_256(cnt, s_warp, &total);
+        const uint32_t local = block_excl_scan<256>(cnt, s_warp, &total);
         if (MR.small_list) {   // the heads' size classes, in head order
             uint32_t o = local;
 #pragma unroll
@@ -550,46 +550,57 @@ __global__ void __launch_bounds__(PS_THREADS, 1) k_part_scatter(const int32_t* _
 
 // One partition per CTA iteration (partitions taken by ticket, in order):
 //   1. 256-bp bucket histogram of the partition in shared memory, its pairs read from its pages (below)
-//   2. one pass over every thread's strip of BP / 256 consecutive buckets: keep flags by a sliding +-rb window (the halo
-//      taken from the neighbours' edge counts -- the same rule as a genome-wide histogram; strips whose windows stay
-//      inside the partition and reach only the neighbouring strips skip the halo tests) and the strip's survivors;
-//      one CTA scan gives the partition's survivor total, published to the look-back at once, and every strip's base
+//   2. one pass over every thread's strip of PER = BP / PF_THREADS consecutive buckets: keep flags by a sliding +-rb
+//      window (the halo taken from the neighbours' edge counts -- the same rule as a genome-wide histogram; strips whose
+//      windows stay inside the partition and reach only the neighbouring strips skip the halo tests) and the strip's
+//      survivors; one CTA scan gives the partition's survivor total, published to the look-back at once, and every
+//      strip's base
 //   3. a second pass over the strip writes the exclusive offsets of the kept buckets and their flag bits; the pairs are
 //      streamed again and every survivor is put into its bucket's slot range in the shared-memory stage (more than
 //      PF_STAGE survivors: in `spill`, at the output's offsets)
-//   4. order inside every bucket: rank against the bucket (<= FIX_SMALL members), or a CTA counting sort on the low
+//   4. order inside every bucket: rank against the bucket (<= FIX_SMALL members), or a counting sort on the low
 //      BKT_SHIFT bits for larger buckets -> keys_out / idx_out at the partition's survivor base
-// Bucket b is stored transposed, at phys(b) = (b % per) * 256 + b / per (per = BP / 256 buckets per strip), so the 256
-// threads reading the j-th bucket of their strips touch 256 consecutive words.  The look-back's exclusive base is
-// awaited only where it is used: before the placement of a partition that spills, otherwise by warp 0 before its share
-// of the placement, while the other warps place theirs.
-// Both passes read the partition's ordinals e = 2 * thread, 2 * thread + 512, .. two pairs (16 B) at a time, U loads in
-// flight per thread: pool page pt[p][e / PART_PAGE] - 1, slot e % PART_PAGE.  The page ids are read through L1: row p of
-// the page table is read and reset by this CTA only.  Once both passes are done the CTA zeroes fill[p] and the entries
-// of row p it read, which are exactly the ones the scatter set, so the next call starts from a clean table.
-__global__ void __launch_bounds__(256) k_part_filter(const uint2* __restrict__ pool, uint32_t* __restrict__ fill, uint32_t* __restrict__ pt,
+// Bucket b is stored transposed, at phys(b) = (b % PER) * PF_THREADS + b / PER, so the threads reading the j-th bucket
+// of their strips touch consecutive words.  Below PF_THREADS buckets (W = 16, BP = 256) PER is 1 and the threads at or
+// past BP own an empty strip: run_indel's choice of W, and with it the partitions, stays what it is for small genomes,
+// and the threads without a strip still load pairs and place survivors.  The look-back's exclusive base is awaited only
+// where it is used: before the placement of a partition that spills, otherwise by warp 0 before its share of the
+// placement, while the other warps place theirs.
+// Both passes read the partition's ordinals e = 2 * thread, 2 * thread + 2 * PF_THREADS, .. two pairs (16 B) at a time,
+// U loads in flight per thread: pool page pt[p][e / PART_PAGE] - 1, slot e % PART_PAGE.  One CTA step covers four pages,
+// load u of a thread lying in page u / 2 of the step.  The page ids are read through L1: row p of the page table is read
+// and reset by this CTA only.  Once both passes are done the CTA zeroes fill[p] and the entries of row p it read, which
+// are exactly the ones the scatter set, so the next call starts from a clean table.
+// 512 threads and 64 registers at most: two CTAs per SM fill its shared memory and its register file.
+static constexpr int PF_THREADS = 512, PF_LT = 9;
+static_assert(PF_THREADS == 1 << PF_LT, "k_part_filter: a power-of-two CTA");
+static_assert((1 << (PART_W_MAX - BKT_SHIFT)) / PF_THREADS <= 64, "k_part_filter: a strip's keep flags fit one 64-bit word");
+static_assert((1 << (PART_W_MIN - BKT_SHIFT)) % 32 == 0,
+              "k_part_filter: below PF_THREADS buckets, one bucket per thread; whole warps own a strip or none");
+__global__ void __launch_bounds__(PF_THREADS, 2) k_part_filter(const uint2* __restrict__ pool, uint32_t* __restrict__ fill, uint32_t* __restrict__ pt,
                                                      uint32_t ptw, int P, int W, int rb, uint32_t need, const uint32_t* __restrict__ edge, uint32_t* __restrict__ keys_out,
                                                      uint32_t* __restrict__ idx_out, uint2* __restrict__ spill, uint32_t* n_out, TileSync ts) {
     pdl_launch_dependents(); pdl_wait();
     extern __shared__ __align__(16) uint32_t s_dyn[];
-    const int BP = 1 << (W - BKT_SHIFT), LPER = W - BKT_SHIFT - 8, PER = 1 << LPER;   // PER buckets per strip
+    const int BP = 1 << (W - BKT_SHIFT);
+    const int LPER = W - BKT_SHIFT > PF_LT ? W - BKT_SHIFT - PF_LT : 0, PER = 1 << LPER;   // PER buckets per strip
     uint32_t* s_h = s_dyn;                                        // BP words, bucket b at phys(b)
     uint32_t* s_f = s_dyn + BP;                                   // BP / 32 flag words, bit phys(b) % 32 of word phys(b) / 32
     uint2* s_st = reinterpret_cast<uint2*>(s_dyn + BP + BP / 32); // PF_STAGE pairs
-    __shared__ uint32_t s_warp[9];
+    __shared__ uint32_t s_warp[PF_THREADS / 32 + 1];
     __shared__ uint32_t s_hl[BKT_PAD], s_hr[BKT_PAD];
     __shared__ uint32_t s_big[PF_BIG_CAP], s_cnt[256];
     __shared__ uint32_t s_tile, s_excl, s_nbig;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t gen = ts_gen(ts);
     const uint32_t bmask = BP - 1;
-    static_assert(PART_W_MIN - BKT_SHIFT >= 8 && PART_W_MAX - BKT_SHIFT <= 14, "one strip of 1..64 buckets per thread");
-    auto phys = [&](uint32_t b) -> uint32_t { return ((b & (PER - 1)) << 8) | (b >> LPER); };
+    auto phys = [&](uint32_t b) -> uint32_t { return ((b & (PER - 1)) << PF_LT) | (b >> LPER); };
     auto count = [&](int b) -> uint32_t { return s_h[phys(b)]; };
-    const int b0 = (int)threadIdx.x * PER;   // this thread's strip
+    const int b0 = (int)threadIdx.x * PER;                 // this thread's strip ..
+    const int nst = (int)threadIdx.x < BP ? PER : 0;       // .. of nst buckets (uniform across a warp)
     while (true) {
         if (threadIdx.x == 0) { s_tile = atomicAdd(ts.ticket, 1u); s_nbig = 0; }
-        for (int i = threadIdx.x; i < BP; i += 256) s_h[i] = 0;
+        for (int i = threadIdx.x; i < BP; i += PF_THREADS) s_h[i] = 0;
         __syncthreads();
         const int p = (int)s_tile;
         if (p >= P) break;
@@ -602,22 +613,23 @@ __global__ void __launch_bounds__(256) k_part_filter(const uint2* __restrict__ p
         const uint32_t np = __ldcg(fill + p);
         uint32_t* row = pt + (size_t)p * ptw;
         auto walk = [&](auto f) {
-            constexpr int U = 8;   // 16 B loads in flight per thread: a step of the CTA covers pages k and k + 1 exactly
-            static_assert(2 * 256 * U == 2 * PART_PAGE, "k_part_filter: two pages per step");
-            for (uint32_t k = 0; 2 * PART_PAGE * k < np; k++) {
-                const uint32_t e0 = 2 * PART_PAGE * k + 2 * threadIdx.x;
-                const uint2* pg0 = pool + (size_t)(__ldg(row + 2 * k) - 1u) * PART_PAGE;
-                const uint2* pg1 = PART_PAGE * (2 * k + 1) < np ? pool + (size_t)(__ldg(row + 2 * k + 1) - 1u) * PART_PAGE : pg0;
+            constexpr int U = 8;   // 16 B loads in flight per thread: a step of the CTA covers pages 4k .. 4k + 3 exactly
+            static_assert(2 * PF_THREADS * U == 4 * PART_PAGE && 2 * PF_THREADS * 2 == PART_PAGE, "k_part_filter: four pages per step, two loads per page");
+            for (uint32_t k = 0; 4 * PART_PAGE * k < np; k++) {
+                const uint32_t e0 = 4 * PART_PAGE * k + 2 * threadIdx.x;
+                uint32_t pg[4];   // pool pages of the step (page 4k + i past the partition's last: never read)
+#pragma unroll
+                for (int i = 0; i < 4; i++) pg[i] = PART_PAGE * (4 * k + i) < np ? __ldg(row + 4 * k + i) - 1u : 0u;
                 uint4 v[U];
 #pragma unroll
                 for (int u = 0; u < U; u++) {
-                    const uint32_t e = e0 + 2 * 256 * u;
-                    v[u] = e < np ? __ldg(reinterpret_cast<const uint4*>((2 * 256 * u + 2 * threadIdx.x < PART_PAGE ? pg0 : pg1) + e % PART_PAGE))
+                    const uint32_t e = e0 + 2 * PF_THREADS * u;
+                    v[u] = e < np ? __ldg(reinterpret_cast<const uint4*>(pool + (size_t)pg[u >> 1] * PART_PAGE + e % PART_PAGE))
                                   : make_uint4(0u, 0u, 0u, 0u);
                 }
 #pragma unroll
                 for (int u = 0; u < U; u++) {
-                    const uint32_t e = e0 + 2 * 256 * u;
+                    const uint32_t e = e0 + 2 * PF_THREADS * u;
                     if (e < np) f(make_uint2(v[u].x, v[u].y));
                     if (e + 1 < np) f(make_uint2(v[u].z, v[u].w));
                 }
@@ -627,11 +639,12 @@ __global__ void __launch_bounds__(256) k_part_filter(const uint2* __restrict__ p
         walk([&](uint2 pr) { atomicAdd(&s_h[phys((pr.x >> BKT_SHIFT) & bmask)], 1u); });
         __syncthreads();
         // 2. keep flags of the strip, the partition's survivor total and the strip's first slot.  Interior strips read the
-        // transposed histogram straight: bucket b0 + s * PER + j of the strip s = -1, 0, 1 is at (j << 8) + thread + s.
-        uint32_t kept, S;
-        const uint64_t flags = pf_strip_flags(count, [&](int s, int j) -> uint32_t { return s_h[(j << 8) + (int)threadIdx.x + s]; },
-                                              b0, PER, BP, rb, need, s_hl, s_hr, &kept);
-        const uint32_t first = block_excl_scan_256(kept, s_warp, &S);
+        // transposed histogram straight: bucket b0 + s * PER + j of the strip s = -1, 0, 1 is at (j << PF_LT) + thread + s.
+        uint32_t kept = 0, S;
+        const uint64_t flags = nst ? pf_strip_flags(count, [&](int s, int j) -> uint32_t { return s_h[(j << PF_LT) + (int)threadIdx.x + s]; },
+                                                    b0, PER, BP, rb, need, s_hl, s_hr, &kept)
+                                   : 0ull;
+        const uint32_t first = block_excl_scan<PF_THREADS>(kept, s_warp, &S);
         if (threadIdx.x == 0) {
             lookback_publish(ts.status, gen, p, S);
             if (S) atomicAdd(n_out, S);
@@ -642,11 +655,11 @@ __global__ void __launch_bounds__(256) k_part_filter(const uint2* __restrict__ p
             if (lane == 0) s_excl = ex;
         }
         // 3a. exclusive offsets of the kept buckets in place, their flag bits, the list of large buckets
-        pf_strip_offsets([&](int b) -> uint32_t { return s_h[((b - b0) << 8) | threadIdx.x]; }, b0, PER, flags, first,
+        pf_strip_offsets([&](int b) -> uint32_t { return s_h[((b - b0) << PF_LT) | threadIdx.x]; }, b0, nst, flags, first,
                          [&](int j, uint32_t off, bool f, uint32_t c) {
-            s_h[(j << 8) | threadIdx.x] = off;   // phys(b0 + j)
+            s_h[(j << PF_LT) | threadIdx.x] = off;   // phys(b0 + j)
             const uint32_t bits = __ballot_sync(0xffffffffu, f);
-            if (lane == 0) s_f[(j << 3) | warp] = bits;
+            if (lane == 0) s_f[(j << (PF_LT - 5)) | warp] = bits;
             if (c > FIX_SMALL) {
                 const uint32_t q = atomicAdd(&s_nbig, 1u);
                 if (q < PF_BIG_CAP) s_big[q] = (uint32_t)(b0 + j);
@@ -664,11 +677,11 @@ __global__ void __launch_bounds__(256) k_part_filter(const uint2* __restrict__ p
             if ((s_f[ph >> 5] >> (ph & 31)) & 1u) st[atomicAdd(&s_h[ph], 1u)] = pr;
         });
         __syncthreads();   // every page id and pair read
-        for (uint32_t k = threadIdx.x; k < (np + PART_PAGE - 1) / PART_PAGE; k += 256) row[k] = 0u;
+        for (uint32_t k = threadIdx.x; k < (np + PART_PAGE - 1) / PART_PAGE; k += PF_THREADS) row[k] = 0u;
         if (threadIdx.x == 0) fill[p] = 0u;
         const uint32_t obase = s_excl;
         // 4a. small buckets: rank against the bucket, ties by slot
-        for (uint32_t q = threadIdx.x; q < S; q += 256) {
+        for (uint32_t q = threadIdx.x; q < S; q += PF_THREADS) {
             const uint2 pr = st[q];
             const uint32_t b = (pr.x >> BKT_SHIFT) & bmask;
             const uint32_t beg = b ? s_h[phys(b - 1)] : 0u, end = s_h[phys(b)];
@@ -681,8 +694,8 @@ __global__ void __launch_bounds__(256) k_part_filter(const uint2* __restrict__ p
             keys_out[obase + beg + rank] = pr.x;
             idx_out[obase + beg + rank] = pr.y;
         }
-        // 4b. large buckets: counting sort on the low BKT_SHIFT bits, one bucket at a time
-        static_assert((1 << BKT_SHIFT) == 256, "one counting-sort bin per thread");
+        // 4b. large buckets: counting sort on the low BKT_SHIFT bits, one bucket at a time; the bins are threads 0 .. 255's
+        static_assert((1 << BKT_SHIFT) == 256 && PF_THREADS >= 256, "one counting-sort bin per thread of the first 256");
         const uint32_t nbig = s_nbig;
         const uint32_t nb = nbig <= (uint32_t)PF_BIG_CAP ? nbig : (uint32_t)BP;   // list overflow: visit every bucket
         for (uint32_t k = 0; k < nb; k++) {
@@ -690,15 +703,15 @@ __global__ void __launch_bounds__(256) k_part_filter(const uint2* __restrict__ p
             const uint32_t beg = b ? s_h[phys(b - 1)] : 0u, end = s_h[phys(b)];
             if (end - beg <= FIX_SMALL) continue;   // (uniform across the CTA)
             __syncthreads();
-            s_cnt[threadIdx.x] = 0;
+            if (threadIdx.x < 256) s_cnt[threadIdx.x] = 0;
             __syncthreads();
-            for (uint32_t j = beg + threadIdx.x; j < end; j += 256) atomicAdd(&s_cnt[st[j].x & 255u], 1u);
+            for (uint32_t j = beg + threadIdx.x; j < end; j += PF_THREADS) atomicAdd(&s_cnt[st[j].x & 255u], 1u);
             __syncthreads();
             uint32_t total;
-            const uint32_t ex = block_excl_scan_256(s_cnt[threadIdx.x], s_warp, &total);
-            s_cnt[threadIdx.x] = ex;
+            const uint32_t ex = block_excl_scan<PF_THREADS>(threadIdx.x < 256 ? s_cnt[threadIdx.x] : 0u, s_warp, &total);
+            if (threadIdx.x < 256) s_cnt[threadIdx.x] = ex;
             __syncthreads();
-            for (uint32_t j = beg + threadIdx.x; j < end; j += 256) {
+            for (uint32_t j = beg + threadIdx.x; j < end; j += PF_THREADS) {
                 const uint2 pr = st[j];
                 const uint32_t d = obase + beg + atomicAdd(&s_cnt[pr.x & 255u], 1u);
                 keys_out[d] = pr.x;

@@ -66,7 +66,7 @@ __global__ void __launch_bounds__(256) k_rs_hist_scan(uint32_t* hist, int passes
     for (int p = 0; p < passes; p++) {
         const uint32_t v = hist[p * 256 + threadIdx.x];
         uint32_t total;
-        const uint32_t e = block_excl_scan_256(v, s_warp, &total);
+        const uint32_t e = block_excl_scan<256>(v, s_warp, &total);
         hist[p * 256 + threadIdx.x] = e;
     }
 }
@@ -141,7 +141,7 @@ __global__ void __launch_bounds__(RS_THREADS, 4) k_rs_onesweep(const K* __restri
             sum += t;
         }
         uint32_t total;
-        const uint32_t excl_local = block_excl_scan_256(sum, s_scan, &total);
+        const uint32_t excl_local = block_excl_scan<256>(sum, s_scan, &total);
         s_excl[d] = excl_local;
         // chained scan of this digit's count over tiles: thread d walks back over the tiles,
         // LB_BATCH predecessors per step (independent loads in flight), so that a wave of W
